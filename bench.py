@@ -2,6 +2,7 @@
 """bench.py -- headline benchmark (contract in the task statement; layout in DESIGN.md section 5).
 
     python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--no-extras] [--step-path module|functional]
+                    [--dump-outputs DIR]
     python -m torch.distributed.run --nnodes=1 --nproc-per-node N ... bench.py --gpus N ...
 
 One "step" = Correlation forward + backward (both input gradients) at BASELINE.json configs[1]:
@@ -14,10 +15,14 @@ e2e          : same metric with HOST buffers: every step copies f1,f2,gradOutput
                memory and copies output,gradInput1,gradInput2 back, through the package's
                hostpipe.HostPipeline (H2D / kernels / D2H of consecutive steps overlap on three streams).
 roofline     : the dominant kernel (correlation backward) timed alone with CUDA events; achieved =
-               its algorithmic bytes per launch / its duration, against MEASURED_PEAKS.json's HBM GB/s.
+               its algorithmic bytes per launch / its duration, against MEASURED_PEAKS.json's HBM GB/s when present,
+               else the H100 SXM data-sheet 3350 GB/s.
+--dump-outputs DIR: after the timed steps, what the last timed step returned (output, grad_input1, grad_input2) as
+               DIR/<name>.npy, float32, each a fixed seeded sample of DUMP_SAMPLE elements (the full tensors are
+               hundreds of MB); the inputs are seeded, so two builds can be compared output for output.
 cpu_baseline : the CPU oracle (oracle/oracle.c, a port -- the reference has no CPU path) on a 1-sample
                slice of the same workload, all host cores.
---impl reference: the reference's OWN CUDA kernels rebuilt for sm_100a (oracle/_ref) on the same
+--impl reference: the reference's OWN CUDA kernels rebuilt for sm_90a (oracle/_ref) on the same
                workload on the same GPU; if they are not built, the CPU oracle port instead.
 flownet2     : image-pairs/s of the unmodified reference models (random weights, 448x1024, bs 8 per GPU) on our
                drop-in layers and through flownet2_b200.fused (glue folded into our kernels); `agreement` = max|d|/max|ref|
@@ -56,12 +61,12 @@ def measured_peak():
     try:
         return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md)"
+        return 3350.0, "H100 SXM data sheet (not measured)"
 
 
 class ClockSampler:
     """SM clock / throttle reasons sampled DURING the timed region (NVML in a thread, 5 ms period;
-    falls back to the nvidia-smi loop of B200_PROFILING.md when pynvml is unusable)."""
+    falls back to an nvidia-smi query loop when pynvml is unusable)."""
     REASONS = {0x8: "hw_slowdown", 0x40: "hw_thermal_slowdown", 0x20: "sw_thermal_slowdown", 0x4: "sw_power_cap"}
 
     def __init__(self, cuda_index):
@@ -212,19 +217,20 @@ def numa_bind(local):
         return {"node": None, "error": str(e)[:100]}
 
 
-def profiled_traffic():
-    """dram__bytes_read+write per launch of the correlation kernels from a COMMITTED ncu capture (profiles/ncu_traffic.json),
-    valid only for the library sources it was taken on: keyed by the product source digest.  None when stale / absent."""
-    try:
-        digest = load_by_path("_fn2_build", "build.py").product_digest()
-        table = json.load(open(os.path.join(ROOT, "profiles", "ncu_traffic.json")))
-        ent = table.get(digest)
-        if ent:
-            ent = dict(ent)
-            ent["digest"] = digest
-        return ent
-    except Exception:
-        return None
+DUMP_SAMPLE = 4 << 20
+
+
+def dump_outputs(out_dir, arrays):
+    """Each array as DIR/<name>.npy: float32 values at DUMP_SAMPLE flat indices drawn with a fixed seed (the same
+    indices for every build and run of the same shape); 3 x 16 MB in all."""
+    import numpy as np
+    import torch
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        flat = t.detach().reshape(-1)
+        idx = torch.randint(0, flat.numel(), (min(DUMP_SAMPLE, flat.numel()),), generator=torch.Generator().manual_seed(0))
+        idx = idx.sort().values.to(flat.device)
+        np.save(os.path.join(out_dir, name + ".npy"), flat[idx].float().cpu().numpy())
 
 
 def load_host_pipeline(impl):
@@ -457,7 +463,7 @@ def extras_ours(dev):
     rec("channelnorm_fwd_c3_fp16", lambda i: (lambda: F2.channelnorm_forward(himgs[i], out=ho1[i])), hw * 2)
     rec("channelnorm_bwd_c3_fp16", lambda i: (lambda: F2.channelnorm_backward(himgs[i], ho1[i], ho1[(i + 1) % NS], out=ho3[i])), hw * 4)
     del himgs, ho1, ho3
-    # hot L2 (the same buffer set every launch; working sets of 117-191 MB vs 126 MB of L2: partly resident)
+    # hot L2 (the same buffer set every launch; working sets of 117-191 MB vs 50 MB of L2: partly resident)
     rec("resample2d_fwd_hotL2", lambda i: (lambda: F2.resample2d_forward(imgs[0], flows[0], out=o3[0])), hw * 8)
     rec("resample2d_bwd_hotL2", lambda i: (lambda: F2.resample2d_backward(imgs[0], flows[0], gos[0], out1=o3[0], out2=o2[0])), hw * 13)
     rec("channelnorm_fwd_c3_hotL2", lambda i: (lambda: F2.channelnorm_forward(imgs[0], out=o1[0])), hw * 4)
@@ -532,6 +538,7 @@ def main():
     ap.add_argument("--flow-ref", nargs="+", metavar=("OUT_DIR", "MODEL"), help=argparse.SUPPRESS)
     ap.add_argument("--step-path", default="module", choices=["module", "functional"],
                     help="ours arm: time the nn.Module + autograd step (default, the call a user makes) or the functional C-ABI calls")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step returned to DIR/<name>.npy")
     args = ap.parse_args()
     args.warmup = max(args.warmup, 3)
     if args.flow_ref:                      # child of the ours arm: reference-kernel output flows for the agreement check
@@ -586,6 +593,7 @@ def main():
         if dist:
             dist.barrier()
 
+    last = {}                              # what the most recent step returned (--dump-outputs)
     if args.impl == "ours" and args.step_path == "module":
         # the call a user makes: the nn.Module (autograd Function) forward, then backward of both input gradients;
         # the Function keeps the forward's bf16 hi/lo workspace for its backward
@@ -596,12 +604,14 @@ def main():
 
         def step():
             o = corr(f1, f2)
-            torch.autograd.grad(o, (f1, f2), gO)
+            gi1, gi2 = torch.autograd.grad(o, (f1, f2), gO)
+            last.update(output=o, grad_input1=gi1, grad_input2=gi2)
         step_how = "flownet2_b200.Correlation module forward + autograd backward (torch.autograd.grad), both input gradients"
     else:
         def step():
             fwd(f1, f2, out)
             bwd(f1, f2, gO, g1, g2)
+            last.update(output=out, grad_input1=g1, grad_input2=g2)
         step_how = ("flownet2_b200.functional.correlation_forward + correlation_backward (workspace handed over)" if args.impl == "ours"
                     else "correlation_cuda.forward + correlation_cuda.backward of the reference extension")
 
@@ -609,15 +619,14 @@ def main():
     if rank == 0:
         sampler.start()
     K, Wm = args.steps, args.warmup
-    steps_cap = None
-    if args.impl == "reference":
-        steps_cap = 5            # the reference backward takes ~0.4 s per step: keep the arm within minutes
-        K = min(K, steps_cap)
     l0 = launches()
     step()
     launches_timed = (launches() - l0) * K      # kernels launched per step x timed steps
     ms, t0, t1 = time_loop(step, K, Wm, sync, barrier if dist else None)
     clocks = sampler.window(t0, t1) if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
+    last.clear()
 
     # dominant-kernel timing (alone, same stream): forward kernel, backward kernels
     f1, f2 = f1.detach(), f2.detach()
@@ -720,26 +729,11 @@ def main():
         else:
             launch_ms = per_f
             ach = fwd_b / (per_f * 1e-3) / 1e9
-        # DRAM traffic per launch: from the committed ncu capture IF it was taken on exactly these library sources
-        # (profiles/ncu_traffic.json keyed by the source digest); never attached to the reference arm; null when stale.
-        prof = profiled_traffic() if args.impl == "ours" else None
-        traffic = traffic_fwd = None
-        if prof:
-            traffic = prof.get("corr_bwd_tc_kernel") if dominant == "correlation_backward" else (
-                (prof.get("corr_fwd_tc_kernel") or 0) + (prof.get("corr_tc_split_kernel") or 0) or None)
-            if prof.get("corr_fwd_tc_kernel") and prof.get("corr_tc_split_kernel"):
-                traffic_fwd = prof["corr_fwd_tc_kernel"] + prof["corr_tc_split_kernel"]
         roofline = {"bound": "hbm", "kernel": kname, "achieved": round(ach, 1), "peak": peak, "unit": "GB/s",
-                    "frac": round(ach / peak, 4), "traffic": traffic,
-                    "traffic_source": ("dram__bytes_read.sum + dram__bytes_write.sum per launch, ncu --set full, %s (sources %s)"
-                                       % (prof.get("source", "profiles/"), prof["digest"][:12])) if prof else
-                                      "no committed ncu capture matches these library sources (profiles/ncu_traffic.json)",
-                    "traffic_forward_incl_split_pass": traffic_fwd,
+                    "frac": round(ach / peak, 4),
                     "algorithmic_bytes": bwd_b if dominant == "correlation_backward" else fwd_b,
                     "peak_source": peak_src, "launch_ms": round(launch_ms, 4),
                     "fp32_tflops": round((51.79e9 * 3) / ((per_f + per_b) * 1e-3) / 1e12, 2)}
-        if prof and prof.get("note"):
-            roofline["note"] = prof["note"]
         line = {
             "metric": "correlation_fwd_bwd_algorithmic_GBps", "value": round(value, 2), "unit": "GB/s",
             "n_gpus": world, "steps": K, "warmup": Wm, "ms_per_step": round(ms / K, 4),
@@ -747,7 +741,7 @@ def main():
             "higher_is_better": True, "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": "Correlation(pad=20,k=1,md=20,s1=1,s2=2) fwd+bwd on fp32 [8,256,112,256] per GPU "
                                    "(BASELINE configs[1])", "per_gpu_batch": B, "global_batch": B * world,
-                       "l2": "inputs+outputs 1.75 GB per step >> 126 MB L2 (no flush needed)",
+                       "l2": "inputs+outputs 1.75 GB per step >> 50 MB L2 (no flush needed)",
                        "parallelism": "replicas x%d (weak, no data-path collective)" % world, "impl": name,
                        "step": step_how},
             "frac_hbm_peak": round(value / world / peak, 4),
@@ -765,8 +759,7 @@ def main():
         }
         if args.impl == "reference":
             line["impl"] = "reference"
-            line["config"]["impl"] = "reference CUDA kernels rebuilt for sm_100a (oracle/_ref)"
-            line["steps_requested"], line["steps_cap"] = args.steps, steps_cap
+            line["config"]["impl"] = "reference CUDA kernels rebuilt for sm_90a (oracle/_ref)"
         if world == 1:
             try:
                 line["cpu_baseline"] = cpu_baseline_sample()

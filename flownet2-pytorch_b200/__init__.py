@@ -1,4 +1,4 @@
-"""flownet2-pytorch_b200 -- B200-native (sm_100a) Correlation / Resample2d / ChannelNorm.
+"""flownet2-pytorch_b200 -- H100-native (sm_90a) Correlation / Resample2d / ChannelNorm.
 
 Import it as ``flownet2_b200`` (the directory name carries a hyphen; ``flownet2_b200.py`` at the
 repo root aliases it).  Public surface = the reference's (networks/*_package/*.py):

@@ -29,7 +29,7 @@ def _load():
         if not os.path.isfile(LIB_PATH):
             raise ImportError(
                 "libfn2b200.so not found at %s -- build it with `python flownet2-pytorch_b200/build.py` "
-                "(needs nvcc, sm_100a). There is no CPU/PyTorch fallback." % LIB_PATH)
+                "(needs nvcc, sm_90a). There is no CPU/PyTorch fallback." % LIB_PATH)
     lib = ctypes.CDLL(LIB_PATH)
     lib.fn2b200_version.restype = _c_int
     lib.fn2b200_last_error.restype = ctypes.c_char_p

@@ -1,10 +1,10 @@
-"""Build libfn2b200.so (the product) and libfn2b200_test.so (hardware self-tests and micro-benchmarks, csrc_test/) for
-sm_100a in-tree with nvcc -- no torch dependency, seconds per file.
+"""Build libfn2b200.so (the product) and libfn2b200_test.so (micro-benchmarks, csrc_test/) for
+sm_90a in-tree with nvcc -- no torch dependency, seconds per file.
 
     python flownet2-pytorch_b200/build.py [--force] [--verbose]
 
-The shared object lands next to this file (git-ignored, but it travels to the GPU box with the
-gpurun snapshot).  Sources are hashed so a rebuild only happens when something changed.
+The shared objects land next to this file (git-ignored build products).  Sources are hashed so a rebuild only happens
+when something changed.
 """
 import hashlib
 import os
@@ -21,7 +21,7 @@ LIB_TEST = os.path.join(HERE, "libfn2b200_test.so")
 STAMP = os.path.join(HERE, "build", "stamp.txt")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC,-O3",
     "-Xptxas", "-v",
@@ -37,21 +37,15 @@ def _test_sources():
     return sorted(f for f in os.listdir(CSRC_TEST) if f.endswith(".cu"))
 
 
-def _digest(product_only=False):
-    """sha1 over the sources and flags; product_only = the digest of what libfn2b200.so is built from (bench.py keys the
-    committed ncu figures in profiles/ on it)."""
+def _digest():
+    """sha1 over the sources and flags."""
     h = hashlib.sha1()
     for f in sorted(os.listdir(CSRC)) + ["../../include/fn2b200.h"]:
         h.update(open(os.path.join(CSRC, f), "rb").read())
-    if not product_only:
-        for f in sorted(os.listdir(CSRC_TEST)):
-            h.update(open(os.path.join(CSRC_TEST, f), "rb").read())
+    for f in sorted(os.listdir(CSRC_TEST)):
+        h.update(open(os.path.join(CSRC_TEST, f), "rb").read())
     h.update(" ".join(NVCC_FLAGS).encode())
     return h.hexdigest()
-
-
-def product_digest():
-    return _digest(product_only=True)
 
 
 def nvcc_path():
@@ -89,7 +83,7 @@ def build(force=False, verbose=False):
 
     def link(out, objects):
         tmp = out + ".tmp%d" % os.getpid()
-        cmd = [nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", tmp] + objects + ["-cudart", "static"]
+        cmd = [nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", tmp] + objects + ["-cudart", "static"]
         r = subprocess.run(cmd, stdout=subprocess.PIPE, stderr=subprocess.STDOUT, text=True)
         if r.returncode != 0:
             raise RuntimeError("link failed:\n" + r.stdout[-4000:])
@@ -99,7 +93,6 @@ def build(force=False, verbose=False):
     # the test library carries its own copy of the host plumbing (runtime.o) -- it never links the product kernels
     link(LIB_TEST, objs[n:] + [os.path.join(obj_dir, "runtime.o")])
     open(STAMP, "w").write(digest)
-    open(os.path.join(obj_dir, "product_digest.txt"), "w").write(product_digest())
     return LIB
 
 

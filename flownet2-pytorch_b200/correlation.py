@@ -1,7 +1,7 @@
 """Correlation (cost-volume) layer -- drop-in for networks/correlation_package/correlation.py.
 
 Same class names, constructor arguments, ``Function.apply`` argument order and defaults as the
-reference (correlation.py:8-60); the arithmetic runs in libfn2b200's sm_100a kernels.
+reference (correlation.py:8-60); the arithmetic runs in libfn2b200's sm_90a kernels.
 """
 import torch
 from torch.autograd import Function

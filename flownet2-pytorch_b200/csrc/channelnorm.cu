@@ -3,7 +3,7 @@
 // Replaces kernel_channelnorm_update_output / kernel_channelnorm_backward_input1
 // (reference channelnorm_package/channelnorm_kernel.cu:18-60, :63-96).
 //
-// B200 design: pure streaming, 0.2-0.5 FLOP/B -> HBM-bound.  One thread owns 4 consecutive pixels:
+// Design: pure streaming, 0.2-0.5 FLOP/B -> HBM-bound.  One thread owns 4 consecutive pixels:
 // C independent 128-bit read-once loads (L1 no-allocate) are issued back to back before any use,
 // so each SM keeps >= 2048 thr x C x 16 B in flight (enough for ~6.6 TB/s at ~600 ns latency),
 // then one 128-bit store.  No shared memory, no pre-zeroed outputs (the reference zero-fills

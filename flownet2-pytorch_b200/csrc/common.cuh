@@ -1,4 +1,4 @@
-// common.cuh -- shared host/device helpers for libfn2b200 (sm_100a only).
+// common.cuh -- shared host/device helpers for libfn2b200 (sm_90a only).
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
@@ -7,8 +7,8 @@
 
 #include "../../include/fn2b200.h"
 
-#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 1000)
-#error "libfn2b200 is written for sm_100a (B200) only"
+#if defined(__CUDA_ARCH__) && (__CUDA_ARCH__ < 900)
+#error "libfn2b200 is written for sm_90a (H100) only"
 #endif
 
 namespace fn2 {
@@ -192,7 +192,7 @@ int corr_forward_tiled(const float *in1, const float *in2, float *out, const Cor
 int corr_backward_tiled(const float *in1, const float *in2, const float *gout, float *gin1,
                         float *gin2, const CorrParams &p, cudaStream_t st);
 
-// Tensor-core (tcgen05) forward for FlowNetC's configuration; needs a caller-provided workspace.
+// Tensor-core (wgmma) forward and backward for FlowNetC's configuration; needs a caller-provided workspace.
 bool corr_tc_supported(const CorrParams &p);
 size_t corr_tc_workspace_bytes(const CorrParams &p);
 int corr_backward_tc(const float *in1, const float *in2, const float *gout, float *gin1, float *gin2,

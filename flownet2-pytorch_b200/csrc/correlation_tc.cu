@@ -1,4 +1,4 @@
-// correlation_tc.cu -- tensor-core (tcgen05 / TMEM) correlation FORWARD and BACKWARD for FlowNetC's configuration
+// correlation_tc.cu -- tensor-core (wgmma) correlation FORWARD and BACKWARD for FlowNetC's configuration
 // (kernel_size 1, stride1 1, stride2 2, displacement radius 10, pad == max_displacement).
 //
 // Formulation (DESIGN.md section 6).  stride2 = 2 means output pixel (y,x) only meets f2 pixels of
@@ -9,21 +9,18 @@
 //        S[p, q] = sum_c f1[c, p] * f2[c, q]        (p in tile, q in halo),
 // computed as a GEMM in 7 "units" of 4 halo rows (N = 144 columns) over K = C channels.
 // fp32 accuracy on bf16 tensor cores: every operand is split x = hi + lo (two bf16, 16 significand
-// bits); S = hi*hi + hi*lo + lo*hi (3 MMAs, fp32 accumulate in TMEM), dropped lo*lo ~ 2^-18 relative.
+// bits); S = hi*hi + hi*lo + lo*hi (3 MMAs, fp32 accumulate in registers), dropped lo*lo ~ 2^-18 relative.
 //
-// Forward pipeline (one persistent CTA per SM, warp-specialised, 416 threads):
+// Forward pipeline (one persistent CTA per SM, warp-specialised, 288 threads):
 //   prepass kernel : NCHW fp32 -> [n][class][yc][xc][c] bf16 hi / lo (channels contiguous = K-major)
-//   warps 0, 10-12 : TMA producers (one batch in flight per warp, so the slots are dealt round-robin):
-//                    f1 tile  -> smem A [hi|lo][C/64][128 rows x 128 B]  (resident for the tile's units)
-//                    f2 units -> smem B ring of 4-5 slots, one slot = hi OR lo of a unit x 64 channels
+//   warp 8         : TMA producer: f1 tile  -> smem A [hi|lo][C/64][128 rows x 128 B]  (resident for the tile's units)
+//                                  f2 units -> smem B ring, one slot = hi OR lo of a unit x 64 channels
 //                    [144 rows x 128 B] = one 18-KB box, 128-byte swizzle; halo outside the image = TMA
 //                    out-of-bounds zero fill = the layer's zero padding
-//   warp 1 (MMA)   : tcgen05.mma.kind::f16 M128 N144 K16; hi slot: hi*hi and lo*hi, lo slot: hi*lo, 4
-//                    k-steps each; accumulators in TMEM (3 buffers x 144 columns), tcgen05.commit -> mbarriers
-//   warps 2-9      : tcgen05.ld the accumulator rows (lane = tile pixel, two warps per lane quadrant), pick
-//                    the 21 band entries of each halo row with a per-lane register shift, scale by 1/C and
-//                    store to out[n][(tj,ti)][y][x]
-#include "umma.cuh"
+//   warps 0-7      : two warpgroups, one per 64 tile pixels: wgmma m64n144k16 (hi slot: hi*hi and lo*hi, lo slot:
+//                    hi*lo, 4 k-steps each) into an fp32 register accumulator, then each thread stores the band entries
+//                    of its fragment, scaled by 1/C, to out[n][(tj,ti)][y][x]
+#include "wgmma.cuh"
 #include <cuda_bf16.h>
 #include <stdlib.h>
 
@@ -38,16 +35,14 @@ constexpr int TC_N = TC_UR * TC_HW;            // 144 accumulator columns per un
 constexpr int TC_KB = 64;                      // channels per k-block (128 B of bf16)
 constexpr int TC_MAXKB = 4;                    // C <= 256
 constexpr int TC_MAXBST = 12;                  // B ring slots (one per hi / lo half-stage): as many as shared memory allows (runtime)
-constexpr int TC_NACC = 3;                     // TMEM accumulator buffers
 constexpr int TC_DS = 2 * TC_DR + 1;           // 21
 constexpr int TC_ABLK = 128 * 128;             // bytes of one A k-block (128 rows x 128 B)
 constexpr int TC_BBLK = TC_N * 128;            // bytes of one B k-block (144 rows x 128 B)
-constexpr int TC_NBAR = 2 * TC_MAXKB + 2 * TC_MAXBST + 2 * TC_NACC;
-constexpr int TC_SMEM_MAX = 232448;                        // 227 KB opt-in limit per CTA
-// dedicated A blocks: hi and lo (SS mode) or lo only (TS mode: the A_hi blocks pass through the B ring on their way
-// to tensor memory), then bst ring slots of one 18-KB box each
-__host__ __device__ constexpr int tc_smem_bytes(int nkb, int bst, bool ts = false) {
-    return (ts ? 1 : 2) * nkb * TC_ABLK + bst * TC_BBLK + TC_NBAR * 8 + 16 + 1024;
+constexpr int TC_NBAR = 2 * TC_MAXKB + 2 * TC_MAXBST;
+constexpr int TC_SMEM_MAX = 232448;            // 227 KB opt-in limit per CTA (sm_90)
+// A_hi and A_lo blocks, then bst ring slots of one 18-KB box each (+ 1 KB for the 1024-byte alignment of the swizzle atoms)
+__host__ __device__ constexpr int tc_smem_bytes(int nkb, int bst) {
+    return 2 * nkb * TC_ABLK + bst * TC_BBLK + TC_NBAR * 8 + 1024;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -144,265 +139,147 @@ __device__ __forceinline__ bool tc_next_seg(int &tn, int &w, int full, int w1, T
     return false;
 }
 
-// One warp keeps only ONE batch of TMA boxes in flight whatever the ring depth (tools/tma_feed.py: 15 B/clk/SM
-// per warp with 18-KB batches, 28 with 36-KB ones, x2 / x4 with 2 / 4 issuing warps, ~75 B/clk/SM ceiling), so
-// the stages are dealt round-robin to `nprod` producer warps: warp 0 and warps 10...
-// Warps: 0 TMA, 1 MMA, 2-9 epilogue (two per TMEM lane quadrant, two halo rows of each unit each), 10.. TMA.
-constexpr int TC_MAXPROD = 4;
-constexpr int TC_EPIWARPS = 8;
-constexpr int TC_THREADS = 64 + 32 * TC_EPIWARPS + 32 * (TC_MAXPROD - 1);
-template <bool TS>
+// Warps 0-7: two consumer warpgroups; warpgroup wg owns tile pixels [64 wg, 64 wg + 64) (tile rows 4 wg .. 4 wg + 3) and
+// keeps their m64 x n144 accumulator of the current unit in registers.  Warp 8: the TMA producer (one lane issues).
+constexpr int TC_CONSUMERS = 256;
+constexpr int TC_THREADS = TC_CONSUMERS + 32;
 __global__ void __launch_bounds__(TC_THREADS, 1)
 corr_fwd_tc_kernel(const __grid_constant__ CUtensorMap m1h, const __grid_constant__ CUtensorMap m1l,
                    const __grid_constant__ CUtensorMap m2h, const __grid_constant__ CUtensorMap m2l,
                    float *__restrict__ out, long out_bstride, float leaky, int B, int C, int H, int W, int ntiles,
-                   int TC_BST, int hint, int nprod, long long *__restrict__ dbg) {
+                   int bst) {
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int Hc = H >> 1, Wc = W >> 1;
     const int nxt = (Wc + TC_TW - 1) / TC_TW, nyt = (Hc + TC_TH - 1) / TC_TH;
     const int nkb = C / TC_KB;
-    // TS: A_hi is copied from shared memory into tensor memory once per tile (tcgen05.cp, columns [288, 288 + C/2))
-    // and the hi x hi and hi x lo products read it from there (TS-mode MMA: 81.5 instead of 112.5 cycles per
-    // M128 x N144 x K16 MMA in isolation, tools/umma_rate.py); the 128 columns come out of the third accumulator buffer.
-    constexpr bool ts = TS;
-    constexpr int nacc = TS ? 2 : TC_NACC;
-    constexpr uint32_t TC_ATM = 2 * TC_N;          // first tensor-memory column of A_hi
-    // Whole tiles round-robin over the CTAs (neighbouring tiles run concurrently and share their halos in L2;
-    // contiguous per-CTA ranges were 50 % slower) for as many full rounds as there are; the tiles of the last,
-    // partial round are dealt out by (tile, unit) pairs -- the 7 units of a tile write disjoint displacement
-    // rows -- so that 1792 tiles on 148 SMs cost 12 rounds + one unit, not 13 rounds.
+    // Whole tiles round-robin over the CTAs (neighbouring tiles run concurrently and share their halos in L2) for as
+    // many full rounds as there are; the tiles of the last, partial round are dealt out by (tile, unit) pairs -- the 7
+    // units of a tile write disjoint displacement rows -- so that the last round costs a few units, not a whole tile.
     const int full = (ntiles / (int)gridDim.x) * (int)gridDim.x;
     const int wtotal = (ntiles - full) * TC_NU, wper = (wtotal + (int)gridDim.x - 1) / (int)gridDim.x;
     const int w0 = (int)blockIdx.x * wper < wtotal ? (int)blockIdx.x * wper : wtotal;
     const int w1 = (w0 + wper < wtotal) ? w0 + wper : wtotal;
     unsigned char *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    // SS: sA = [hi | lo][kb][128 x 128 B].  TS: sA = [lo][kb][128 x 128 B] only -- an A_hi block is needed in shared memory
-    // just long enough to be copied into tensor memory, so it travels through a ring slot like a B stage (16 KB of
-    // the slot's 18 KB), which leaves room for 8 ring slots instead of 5 (1 unit of look-ahead instead of 0.6).
-    unsigned char *sA = smem;
-    unsigned char *sAlo = smem + (TS ? 0 : nkb * TC_ABLK);
-    unsigned char *sB = smem + (TS ? 1 : 2) * nkb * TC_ABLK;    // [slot][144 x 128 B]
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sB + TC_BST * TC_BBLK);
+    unsigned char *sA = smem;                              // A_hi [kb][128 rows x 128 B], resident for a tile's units
+    unsigned char *sAlo = smem + nkb * TC_ABLK;            // A_lo [kb][128 rows x 128 B]
+    unsigned char *sB = smem + 2 * nkb * TC_ABLK;          // ring [slot][144 rows x 128 B]
+    uint64_t *bars = reinterpret_cast<uint64_t *>(sB + bst * TC_BBLK);
     uint64_t *a_full = bars, *a_empty = bars + TC_MAXKB;
     uint64_t *b_full = bars + 2 * TC_MAXKB, *b_empty = b_full + TC_MAXBST;
-    uint64_t *acc_full = b_empty + TC_MAXBST, *acc_empty = acc_full + TC_NACC;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + TC_NBAR);
 
     if (tid == 0) {
         prefetch_tensormap(&m1h); prefetch_tensormap(&m1l);
         prefetch_tensormap(&m2h); prefetch_tensormap(&m2l);
-        for (int i = 0; i < TC_MAXKB; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], 1); }
-        for (int i = 0; i < TC_MAXBST; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 1); }
-        for (int i = 0; i < TC_NACC; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 32 * TC_EPIWARPS); }
+        for (int i = 0; i < TC_MAXKB; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], TC_CONSUMERS); }
+        for (int i = 0; i < TC_MAXBST; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], TC_CONSUMERS); }
         fence_barrier_init();
     }
-    if (warp == 1) tmem_alloc<512>(tmem_slot);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0 || warp >= 2 + TC_EPIWARPS) {
-        // ===================== TMA producers (converged warps, one elected lane issues) =====================
-        const int prod = warp == 0 ? 0 : warp - (1 + TC_EPIWARPS);
-        if (prod < nprod) {
-            uint32_t bcount = 0, job = 0;          // job: every A block / B stage in issue order
+    if (warp == TC_CONSUMERS / 32) {
+        // ===================== TMA producer =====================
+        if (lane == 0) {
+            uint32_t bcount = 0;
             int it = 0;
             const uint64_t pol = l2_policy_evict_last();
-            auto load = [&](void *dst, const CUtensorMap *m, uint64_t *bar, int c0, int c1, int c2, int c3) {
-                if (hint) tma_load_4d_hint(dst, m, bar, c0, c1, c2, c3, pol);
-                else tma_load_4d(dst, m, bar, c0, c1, c2, c3);
-            };
             TcSeg sg;
             for (int tn = blockIdx.x, w = w0; tc_next_seg(tn, w, full, w1, sg); ++it) {
-                const int ua = sg.ua, ub = sg.ub;
                 const TcTile T = tc_decode(sg.t, nxt, nyt);
                 const int img = T.n * 4 + T.py * 2 + T.px;
-                if (TS) {
-                    // the tile's A_hi blocks as ring stages (consumed by tcgen05.cp, first thing in the segment)
-                    for (int kb = 0; kb < nkb; ++kb, ++bcount, ++job) {
-                        if ((int)(job % (uint32_t)nprod) != prod) continue;
-                        const int s = bcount % TC_BST;
-                        mbar_wait(&b_empty[s], ((bcount / TC_BST) & 1) ^ 1);
-                        if (elect_one_sync()) {
-                            mbar_arrive_expect_tx(&b_full[s], TC_ABLK);
-                            load(sB + s * TC_BBLK, &m1h, &b_full[s], kb * TC_KB, T.xc0, T.yc0, img);
-                        }
-                        __syncwarp();
-                    }
-                }
-                for (int kb = 0; kb < nkb; ++kb, ++job) {
-                    if ((int)(job % (uint32_t)nprod) != prod) continue;
+                // the tile's A blocks: one k-block is refilled as soon as the previous segment's last unit has read it
+                for (int kb = 0; kb < nkb; ++kb) {
                     mbar_wait(&a_empty[kb], (it & 1) ^ 1);
-                    if (elect_one_sync()) {
-                        mbar_arrive_expect_tx(&a_full[kb], (TS ? 1 : 2) * TC_ABLK);
-                        if (!TS) load(sA + kb * TC_ABLK, &m1h, &a_full[kb], kb * TC_KB, T.xc0, T.yc0, img);
-                        load(sAlo + kb * TC_ABLK, &m1l, &a_full[kb], kb * TC_KB, T.xc0, T.yc0, img);
-                    }
-                    __syncwarp();
+                    mbar_arrive_expect_tx(&a_full[kb], 2 * TC_ABLK);
+                    tma_load_4d_hint(sA + kb * TC_ABLK, &m1h, &a_full[kb], kb * TC_KB, T.xc0, T.yc0, img, pol);
+                    tma_load_4d_hint(sAlo + kb * TC_ABLK, &m1l, &a_full[kb], kb * TC_KB, T.xc0, T.yc0, img, pol);
                 }
-                // B: one 18-KB box per half-stage (hi, then lo, of one unit x k-block) -- TC_BST slots
-                for (int u = ua; u < ub; ++u)
+                // B: one 18-KB box per half-stage (hi, then lo, of one unit x k-block); halo outside the image = TMA
+                // out-of-bounds zero fill = the layer's zero padding
+                for (int u = sg.ua; u < sg.ub; ++u)
                     for (int kb = 0; kb < nkb; ++kb)
-                        for (int hl = 0; hl < 2; ++hl, ++bcount, ++job) {
-                            if ((int)(job % (uint32_t)nprod) != prod) continue;
-                            const int s = bcount % TC_BST;
-                            mbar_wait(&b_empty[s], ((bcount / TC_BST) & 1) ^ 1);
-                            if (elect_one_sync()) {
-                                mbar_arrive_expect_tx(&b_full[s], TC_BBLK);
-                                load(sB + s * TC_BBLK, hl ? &m2l : &m2h, &b_full[s], kb * TC_KB, T.xc0 - TC_DR,
-                                     T.yc0 - TC_DR + u * TC_UR, img);
-                            }
-                            __syncwarp();
-                        }
-            }
-        }
-    } else if (warp == 1) {
-        // ===================== MMA issuer (converged warp, one elected lane issues) =====================
-        {
-            const uint32_t idesc = umma_idesc_bf16_f32(128, TC_N);
-            uint32_t bcount = 0, acount = 0;
-            int it = 0;
-            TcSeg sg;
-            for (int tn = blockIdx.x, w = w0; tc_next_seg(tn, w, full, w1, sg); ++it) {
-                const int ua = sg.ua, ub = sg.ub;
-                if (TS) {
-                    // A_hi: ring stage -> tensor memory, one K = 16 step per copy.  tcgen05.cp and tcgen05.mma execute in
-                    // issue order: the copies wait for the previous tile's MMAs that still read these columns, the MMAs
-                    // below wait for the copies; the commit frees the ring slot once the copies have read it.
-                    for (int kb = 0; kb < nkb; ++kb, ++bcount) {
-                        const int s = bcount % TC_BST;
-                        mbar_wait(&b_full[s], (bcount / TC_BST) & 1);
-                        tcgen05_fence_after();
-                        if (elect_one_sync()) {
-                            const uint64_t src = umma_desc_k_sw128(smem_u32(sB + s * TC_BBLK));
-                            const uint32_t dst = tmem_base + TC_ATM + kb * (TC_KB / 2);
-#pragma unroll
-                            for (int ks = 0; ks < TC_KB / 16; ++ks) umma_cp_128x256b(dst + ks * 8, src + 2 * ks);
-                            umma_commit(&b_empty[s]);
-                        }
-                        __syncwarp();
-                    }
-                }
-                for (int u = ua; u < ub; ++u, ++acount) {
-                    const int ab = acount % nacc;
-                    const bool rec = dbg && blockIdx.x == 0 && acount < 64 && lane == 0;
-                    long long bwait = 0;
-                    if (rec) dbg[acount * 8 + 0] = clock64();
-                    mbar_wait(&acc_empty[ab], ((acount / nacc) & 1) ^ 1);
-                    if (rec) dbg[acount * 8 + 1] = clock64();
-                    tcgen05_fence_after();
-                    const uint32_t d = tmem_base + ab * TC_N;
-                    for (int kb = 0; kb < nkb; ++kb) {
-                        const uint64_t ah = umma_desc_k_sw128(smem_u32(sA + kb * TC_ABLK));          // SS mode only
-                        const uint64_t al = umma_desc_k_sw128(smem_u32(sAlo + kb * TC_ABLK));
-                        const uint32_t atm = tmem_base + TC_ATM + kb * (TC_KB / 2);
-                        if (u == ua) mbar_wait(&a_full[kb], it & 1);
                         for (int hl = 0; hl < 2; ++hl, ++bcount) {
-                            const int s = bcount % TC_BST;
-                            const long long tw0 = rec ? clock64() : 0;
-                            mbar_wait(&b_full[s], (bcount / TC_BST) & 1);
-                            if (rec) bwait += clock64() - tw0;
-                            tcgen05_fence_after();
-                            if (elect_one_sync()) {
-                                const uint64_t bd = umma_desc_k_sw128(smem_u32(sB + s * TC_BBLK));
-                                if (hl == 0) {
-#pragma unroll
-                                    for (int ks = 0; ks < TC_KB / 16; ++ks) {           // hi x hi, lo x hi
-                                        if (ts) umma_bf16_ts(d, atm + ks * 8, bd + 2 * ks, idesc, (kb | ks) != 0);
-                                        else umma_bf16_ss(d, ah + 2 * ks, bd + 2 * ks, idesc, (kb | ks) != 0);
-                                        umma_bf16_ss(d, al + 2 * ks, bd + 2 * ks, idesc, 1);
-                                    }
-                                } else {
-#pragma unroll
-                                    for (int ks = 0; ks < TC_KB / 16; ++ks) {           // hi x lo
-                                        if (ts) umma_bf16_ts(d, atm + ks * 8, bd + 2 * ks, idesc, 1);
-                                        else umma_bf16_ss(d, ah + 2 * ks, bd + 2 * ks, idesc, 1);
-                                    }
-                                }
-                                umma_commit(&b_empty[s]);                        // slot may be refilled
-                                if (hl == 1) {
-                                    if (u == ub - 1) umma_commit(&a_empty[kb]);     // A block free for the next tile
-                                    if (kb == nkb - 1) umma_commit(&acc_full[ab]);
-                                }
-                            }
-                            __syncwarp();
+                            const int s = bcount % bst;
+                            mbar_wait(&b_empty[s], ((bcount / bst) & 1) ^ 1);
+                            mbar_arrive_expect_tx(&b_full[s], TC_BBLK);
+                            tma_load_4d_hint(sB + s * TC_BBLK, hl ? &m2l : &m2h, &b_full[s], kb * TC_KB, T.xc0 - TC_DR,
+                                             T.yc0 - TC_DR + u * TC_UR, img, pol);
                         }
-                    }
-                    if (rec) { dbg[acount * 8 + 2] = bwait; dbg[acount * 8 + 3] = clock64(); }
-                }
             }
         }
     } else {
-        // ===================== epilogue (warps 2..9) =====================
-        // Thread = accumulator row (tile pixel p); its 21 outputs of halo row hrl are columns
-        // [px_t, px_t + 21) of that row's 36: a per-lane register shift (4 conditional stages of 8/4/2/1)
-        // instead of a round trip through shared memory -- the kernel is bound by shared-memory
-        // bandwidth (MMA operand reads + TMA writes), and the staging rows cost ~1.7K wavefronts per unit.
-        const int quad = warp & 3;                 // TMEM lane quadrant this warp may access
-        const int half = (warp - 2) >> 2;          // halo rows {2 half, 2 half + 1} of every unit
-        const int p = quad * 32 + lane;            // tile pixel = TMEM lane = accumulator row
-        const int py_t = p >> 4, px_t = p & 15;
-        // 1/(k*k*C): exact for power-of-two C (FlowNetC: 256) -> bit-identical to the reference's divide;
-        // otherwise within 1 ulp.  (An IEEE divide here costs a slow-path call + reconvergence barrier
-        // per output and serialises the epilogue: measured 13K cycles per unit.)
+        // ===================== consumers: wgmma + epilogue =====================
+        const int wg = warp >> 2, wq = warp & 3;
+        // accumulator fragment: rows 16 wq + lane / 4 (+ 8) of the warpgroup = tile row 4 wg + wq, columns pxa (+ 8)
+        const int py_t = 4 * wg + wq, pxa = lane >> 2, q = lane & 3;
+        // 1/(k*k*C): exact for power-of-two C (FlowNetC: 256) -> bit-identical to the reference's divide; otherwise
+        // within 1 ulp.
         const float inv_nelems = 1.0f / (float)C;
         const long plane = (long)H * W;
-        const bool s8 = px_t & 8, s4 = px_t & 4, s2 = px_t & 2, s1 = px_t & 1;
         const bool act = leaky != 1.f;
-        uint32_t acount = 0;
+        uint32_t bcount = 0;
+        int it = 0;
         TcSeg sg;
-        for (int tn = blockIdx.x, w = w0; tc_next_seg(tn, w, full, w1, sg);) {
+        for (int tn = blockIdx.x, w = w0; tc_next_seg(tn, w, full, w1, sg); ++it) {
             const int ua = sg.ua, ub = sg.ub;
             const TcTile T = tc_decode(sg.t, nxt, nyt);
-            const int yc = T.yc0 + py_t, xc = T.xc0 + px_t;
-            const bool pix_ok = (yc < Hc) && (xc < Wc);
-            float *obase = out + (long)T.n * out_bstride + (long)(2 * yc + T.py) * W + (2 * xc + T.px);
-            for (int u = ua; u < ub; ++u, ++acount) {
-                const int ab = acount % nacc;
-                const bool rec = dbg && blockIdx.x == 0 && acount < 64 && p == 0 && half == 0;
-                if (rec) dbg[acount * 8 + 4] = clock64();
-                mbar_wait(&acc_full[ab], (acount / nacc) & 1);
-                if (rec) dbg[acount * 8 + 5] = clock64();
-                tcgen05_fence_after();
-#pragma unroll 1
-                for (int hh = 0; hh < 2; ++hh) {
-                    const int hrl = 2 * half + hh;
-                    const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + ab * TC_N + hrl * TC_HW;
-                    float r[TC_HW];
-                    tmem_ld16(taddr, r);
-                    tmem_ld16(taddr + 16, r + 16);
-                    tmem_ld4(taddr + 32, r + 32);
-                    tmem_ld_wait();
+            const int yc = T.yc0 + py_t, xc = T.xc0 + pxa;
+            const bool ok0 = (yc < Hc) && (xc < Wc), ok1 = (yc < Hc) && (xc + 8 < Wc);
+            float *ob = out + (long)T.n * out_bstride + (long)(2 * yc + T.py) * W + (2 * xc + T.px);
+            for (int u = ua; u < ub; ++u) {
+                float acc[TC_N / 2];
 #pragma unroll
-                    for (int j = 0; j < 28; ++j) r[j] = s8 ? r[j + 8] : r[j];
+                for (int i = 0; i < TC_N / 2; ++i) acc[i] = 0.f;
+                wgmma_fence_operands(acc);
+                int prev = -1, prev_a = -1;            // ring slot (and A block) read by the wgmma group in flight
+                for (int kb = 0; kb < nkb; ++kb) {
+                    if (u == ua) mbar_wait(&a_full[kb], it & 1);
+                    const uint64_t dh = wgmma_desc_k_sw128(smem_u32(sA + kb * TC_ABLK + wg * (TC_ABLK / 2)));
+                    const uint64_t dl = wgmma_desc_k_sw128(smem_u32(sAlo + kb * TC_ABLK + wg * (TC_ABLK / 2)));
 #pragma unroll
-                    for (int j = 0; j < 24; ++j) r[j] = s4 ? r[j + 4] : r[j];
+                    for (int hl = 0; hl < 2; ++hl, ++bcount) {
+                        const int s = bcount % bst;
+                        mbar_wait(&b_full[s], (bcount / bst) & 1);
+                        const uint64_t bd = wgmma_desc_k_sw128(smem_u32(sB + s * TC_BBLK));
+                        wgmma_fence();
 #pragma unroll
-                    for (int j = 0; j < 22; ++j) r[j] = s2 ? r[j + 2] : r[j];
-#pragma unroll
-                    for (int j = 0; j < 21; ++j) r[j] = s1 ? r[j + 1] : r[j];
-                    const int tj = u * TC_UR + hrl - py_t;          // = tj + DR, valid in [0, 20]
-                    if (pix_ok && tj >= 0 && tj < TC_DS) {
-                        float *o = obase + (long)(tj * TC_DS) * plane;
-#pragma unroll
-                        for (int ti = 0; ti < TC_DS; ++ti) {
-                            float v = r[ti] * inv_nelems;
-                            if (act) v = v > 0.f ? v : v * leaky;      // fused nn.LeakyReLU (FlowNetC.py:87), warp-uniform
-                            __stcs(o + ti * plane, v);
+                        for (int ks = 0; ks < TC_KB / 16; ++ks) {
+                            wgmma_m64n144k16_k(acc, dh + 2 * ks, bd + 2 * ks);             // hi x hi | hi x lo
+                            if (hl == 0) wgmma_m64n144k16_k(acc, dl + 2 * ks, bd + 2 * ks); // lo x hi
                         }
+                        wgmma_commit();
+                        wgmma_wait<1>();
+                        if (prev >= 0) {
+                            mbar_arrive(&b_empty[prev]);
+                            if (prev_a >= 0) mbar_arrive(&a_empty[prev_a]);
+                        }
+                        prev = s;
+                        prev_a = (hl == 1 && u == ub - 1) ? kb : -1;       // A block free for the next segment
                     }
                 }
-                tcgen05_fence_before();
-                mbar_arrive(&acc_empty[ab]);
-                if (rec) dbg[acount * 8 + 6] = clock64();
+                wgmma_wait<0>();
+                wgmma_fence_operands(acc);
+                mbar_arrive(&b_empty[prev]);
+                if (prev_a >= 0) mbar_arrive(&a_empty[prev_a]);
+                // accumulator column c = hrl * 36 + qx (halo row hrl of the unit, halo column qx) of tile pixel
+                // (py_t, px) is displacement (tj, ti) = (u * 4 + hrl - py_t, qx - px) - (10, 10), if inside the band
+                const int tjb = u * TC_UR - py_t;
+#pragma unroll
+                for (int i = 0; i < TC_N / 8; ++i)
+#pragma unroll
+                    for (int j = 0; j < 4; ++j) {
+                        const int c = 8 * i + 2 * q + (j & 1);
+                        const int hrl = c / TC_HW;
+                        const int ti = c - hrl * TC_HW - pxa - 8 * (j >> 1), tj = tjb + hrl;
+                        if (((j >> 1) ? ok1 : ok0) && (unsigned)ti < (unsigned)TC_DS && (unsigned)tj < (unsigned)TC_DS) {
+                            float v = acc[4 * i + j] * inv_nelems;
+                            if (act) v = v > 0.f ? v : v * leaky;      // fused nn.LeakyReLU (FlowNetC.py:87), warp-uniform
+                            __stcs(ob + 16 * (j >> 1) + (long)(tj * TC_DS + ti) * plane, v);
+                        }
+                    }
             }
         }
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc<512>(tmem_base);
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -410,72 +287,71 @@ corr_fwd_tc_kernel(const __grid_constant__ CUtensorMap m1h, const __grid_constan
 //
 //   gI1[c, p] = 1/C sum_q G1[p, q] f2[c, q],   G1[p, q] = gO[(q - p), p]          (|q - p| <= 10)
 //   gI2[c, q] = 1/C sum_p G2[q, p] f1[c, p],   G2[q, p] = gO[(q - p), p]
-// per parity class: D[128 tile px][C] += A[128][144] * B[144 halo px][C] over the 7 halo-row units,
-// accumulated in ONE TMEM buffer per tile (C <= 256 fp32 columns, double-buffered across tiles).
-//   A = the banded gradOutput matrix, built per unit by 16 "builder" warps straight from the fp32
-//       gradOutput planes (bf16 hi/lo split on the fly) into an MN-major SW128 layout [k][64 pixels]
-//       (K-major layouts made the 2-byte band scatter 4- to 6.5-way bank conflicted, ncu);
-//   B = the other input's halo chunk from the prepass copy ([pixel][channel] bf16 = MN-major operand),
-//       one slot = hi OR lo of a K-group (48 halo pixels) x all channel blocks;
-//   3 MMAs (hi*hi, lo*hi | hi*lo) per k-step, N = C <= 256 per instruction.
-// Roles (768 threads): warps 0, 22, 23 TMA, warp 1 MMA, warps 2-17 builders, warps 18-21 epilogue.
-// Builders: FOUR threads per tile pixel = (halo-row pair) x (displacement half); a single warp per
-// scheduler ran ~2000 dependent instructions per unit at IPC ~0.2 and made the builder -- not the
-// tensor pipe -- the bottleneck.  Loads stay coalesced (lanes = pixels, one displacement plane per
-// instruction); the band positions a pixel row writes are the same for every unit, so the zero
-// columns of A are written ONCE at kernel start and the scatter offsets live in registers.
+// per parity class: D[128 tile px][C] += A[128][144] * B[144 halo px][C] over the 7 halo-row units, accumulated in
+// registers (warpgroup wg: tile pixels [64 wg, 64 wg + 64), an m64 x nC fragment) for the whole tile.
+//   A = the banded gradOutput matrix, built per unit by the warpgroup's own threads straight from the fp32 gradOutput
+//       planes (bf16 hi/lo split on the fly) into an MN-major SW128 layout [k][64 pixels] (two buffers per warpgroup,
+//       so that building unit u + 1 overlaps the last wgmma group of unit u, and each warpgroup's building overlaps
+//       the other's MMAs);
+//   B = the other input's halo chunk from the prepass copy ([pixel][channel] bf16 = MN-major operand), one ring slot =
+//       hi OR lo of a K-group (48 halo pixels) x all channel blocks;
+//   3 products (hi*hi, lo*hi | hi*lo) per k-step, N = C <= 256 per instruction.
+// Two threads per tile pixel build A: halo rows {2 hp, 2 hp + 1} x all 21 displacements each.  Loads stay coalesced
+// (lanes = pixels, one displacement plane per instruction); the band positions a pixel row writes are the same for
+// every unit, so the zero columns of A are written ONCE at kernel start and the scatter offsets live in registers.
 // ------------------------------------------------------------------------------------------------
-constexpr int TB_KS = TC_N / 16;                   // 9 k-steps per unit
-constexpr int TB_AMB = TC_N * 128;                 // 18432 B: one 64-pixel block of A, [k][64 pixels] (MN-major, SW128)
-constexpr int TB_AHL = 2 * TB_AMB;                 // 36864 B: one of {hi, lo} of a unit's A
-// byte offset of A element (tile pixel p, k): pixels contiguous, 16-byte chunk index XOR (k & 7)
+constexpr int TB_AHL = TC_N * 128;                 // 18432 B: hi (or lo) of a warpgroup's A, [k][64 pixels] (MN-major, SW128)
+constexpr int TB_ASTG = 2 * TB_AHL;                // hi + lo
+constexpr int TB_NAST = 2;                         // A buffers per warpgroup
+constexpr int TB_SMEM_A = 2 * TB_NAST * TB_ASTG;   // 147456
+// byte offset of A element (pixel p of the warpgroup's 64, k): pixels contiguous, 16-byte chunk index XOR (k & 7)
 __host__ __device__ constexpr uint32_t tb_a_offset(uint32_t p, uint32_t k) {
-    return (p >> 6) * TB_AMB + k * 128u + (((((p & 63u) >> 3) ^ (k & 7u))) << 4) + (p & 7u) * 2u;
+    return k * 128u + ((((p >> 3) ^ (k & 7u))) << 4) + (p & 7u) * 2u;
 }
-constexpr int TB_ASTG = 2 * TB_AHL;                // 73728 B per A stage
-constexpr int TB_NAST = 2, TB_MAXBST = 6, TB_NACC = 2;
-constexpr int TB_SMEM_A = TB_NAST * TB_ASTG;       // 147456
-constexpr int TB_NBAR = 2 * TB_NAST + 2 * TB_MAXBST + 2 * TB_NACC;
-// B staging: the unit's 144 K indices in 3 groups of 48 (12 halo columns x 4 rows); one half-stage = the
-// hi (or the lo) copy of one group x ALL channel blocks = up to 4 boxes of 6 KB, so every MMA covers N = C
-// columns: both operands come from shared memory (128 B/clk), an M128 x N x K16 MMA reads 4 KB of A and
-// N/32 KB of B, and the kernel is bound by that traffic -- N = 256 reads A half as often as N = 128 did.
+constexpr int TB_MAXBST = 6;
+constexpr int TB_NBAR = 2 * TB_MAXBST;
+// B staging: the unit's 144 K indices in 3 groups of 48 (12 halo columns x 4 rows); one ring slot = the hi (or the lo)
+// copy of one group x ALL channel blocks = up to 4 boxes of 6 KB, so every wgmma covers N = C columns.
 constexpr int TB_NG = 3, TB_GW = TC_HW / TB_NG, TB_GK = TC_UR * TB_GW;   // 3 groups, 12 columns, 48 K
 constexpr int TB_GBLK = TB_GK * 128;               // 6144 B: one 64-channel block of a group's rows
 constexpr int TB_BSTAGE = 4 * TB_GBLK;             // 24576 B: [<= 4 channel blocks][48 rows x 128 B]
 __host__ __device__ constexpr uint32_t tb_kindex(uint32_t hrl, uint32_t qx) {
     return (qx / TB_GW) * TB_GK + hrl * TB_GW + (qx % TB_GW);
 }
-constexpr int TB_MAXPROD = 3;                      // TMA producer warps (one batch in flight each, see the forward)
-constexpr int TB_THREADS = 704 + 32 * (TB_MAXPROD - 1);   // warp 0 TMA, 1 MMA, 2-17 builders, 18-21 epilogue, 22.. TMA
+// warps 0-7: two warpgroups (build A, wgmma, epilogue) with 232 registers a thread (setmaxnreg: the m64 x n256 accumulator
+// alone is 128); warps 8-11: a producer warpgroup lowered to 40 registers, of which warp 8 issues the TMA loads
+constexpr int TB_THREADS = TC_CONSUMERS + 128;
 __host__ __device__ constexpr int tb_smem_bytes(int bst) {
-    return TB_SMEM_A + bst * TB_BSTAGE + TB_NBAR * 8 + 16 + 1024;
+    return TB_SMEM_A + bst * TB_BSTAGE + TB_NBAR * 8 + 1024;
 }
 
+template <int NKB>
+__device__ __forceinline__ void wgmma_bwd(float (&d)[NKB * 32], uint64_t da, uint64_t db);
+template <> __device__ __forceinline__ void wgmma_bwd<1>(float (&d)[32], uint64_t da, uint64_t db) { wgmma_m64n64k16_mn(d, da, db); }
+template <> __device__ __forceinline__ void wgmma_bwd<2>(float (&d)[64], uint64_t da, uint64_t db) { wgmma_m64n128k16_mn(d, da, db); }
+template <> __device__ __forceinline__ void wgmma_bwd<3>(float (&d)[96], uint64_t da, uint64_t db) { wgmma_m64n192k16_mn(d, da, db); }
+template <> __device__ __forceinline__ void wgmma_bwd<4>(float (&d)[128], uint64_t da, uint64_t db) { wgmma_m64n256k16_mn(d, da, db); }
 
 // Both gradients in ONE launch: global tiles [t_begin, t_end) of [0, 2 ntiles).  One gradient only: tile g < ntiles
 // is tile g of gradInput1 (B = input2's halo, maps m2h / m2l), tile g >= ntiles is tile g - ntiles of gradInput2
-// (B = input1's halo); both: g = 2 tile + (0 = gradInput1, 1 = gradInput2).  3584 tiles on 148 SMs waste 3 % in the last round, two launches of 1792 wasted 7 % each.
+// (B = input1's halo); both: g = 2 tile + (0 = gradInput1, 1 = gradInput2).
+template <int NKB>
 __global__ void __launch_bounds__(TB_THREADS, 1)
 corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constant__ CUtensorMap m2l,
                    const __grid_constant__ CUtensorMap m1h, const __grid_constant__ CUtensorMap m1l,
-                   const float *__restrict__ gout, float *__restrict__ gin1, float *__restrict__ gin2, int B, int C,
-                   int H, int W, int ntiles, int t_begin, int t_end, int TB_NBST, int hint, int nprod,
-                   long long *__restrict__ dbg) {
+                   const float *__restrict__ gout, float *__restrict__ gin1, float *__restrict__ gin2, int B,
+                   int H, int W, int ntiles, int t_begin, int t_end, int bst) {
+    constexpr int C = NKB * TC_KB;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
     unsigned char *smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    unsigned char *sA = smem;                          // [stage][hl][9 k-steps][2 chunks][16 groups][8 x 16 B]
-    unsigned char *sB = smem + TB_SMEM_A;              // [stage][hl][2 channel blocks][48 rows x 128 B] (SW128, MN-major)
-    uint64_t *bars = reinterpret_cast<uint64_t *>(sB + TB_NBST * TB_BSTAGE);
-    uint64_t *a_full = bars, *a_empty = a_full + TB_NAST;
-    uint64_t *b_full = a_empty + TB_NAST, *b_empty = b_full + TB_MAXBST;
-    uint64_t *acc_full = b_empty + TB_MAXBST, *acc_empty = acc_full + TB_NACC;
-    uint32_t *tmem_slot = reinterpret_cast<uint32_t *>(bars + TB_NBAR);
+    unsigned char *sA = smem;                          // [warpgroup][buffer][hi | lo][144 k x 128 B]
+    unsigned char *sB = smem + TB_SMEM_A;              // [slot][channel block][48 rows x 128 B] (SW128, MN-major)
+    uint64_t *bars = reinterpret_cast<uint64_t *>(sB + bst * TB_BSTAGE);
+    uint64_t *b_full = bars, *b_empty = bars + TB_MAXBST;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int Hc = H >> 1, Wc = W >> 1;
     const int nxt = (Wc + TC_TW - 1) / TC_TW, nyt = (Hc + TC_TH - 1) / TC_TH;
-    const int ncb = C / TC_KB;
     const long plane = (long)H * W;
     // both gradients requested: even global tiles are gradInput1 tiles, odd ones the gradInput2 tile of the same
     // location, so the two readers of a gradOutput region run side by side and the second one finds it in L2
@@ -484,268 +360,165 @@ corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constan
     if (tid == 0) {
         prefetch_tensormap(&m2h); prefetch_tensormap(&m2l);
         prefetch_tensormap(&m1h); prefetch_tensormap(&m1l);
-        for (int i = 0; i < TB_NAST; ++i) { mbar_init(&a_full[i], 16); mbar_init(&a_empty[i], 1); }   // one arrival per builder warp
-        for (int i = 0; i < TB_MAXBST; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], 1); }
-        for (int i = 0; i < TB_NACC; ++i) { mbar_init(&acc_full[i], 1); mbar_init(&acc_empty[i], 128); }
+        for (int i = 0; i < TB_MAXBST; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], TC_CONSUMERS); }
         fence_barrier_init();
     }
     // columns of A outside a pixel row's band are zero for every unit: written once, here
     for (int i = tid; i < TB_SMEM_A / 16; i += TB_THREADS) reinterpret_cast<uint4 *>(sA)[i] = make_uint4(0, 0, 0, 0);
     fence_proxy_async();
-    if (warp == 1) tmem_alloc<512>(tmem_slot);
-    tcgen05_fence_before();
     __syncthreads();
-    tcgen05_fence_after();
-    const uint32_t tmem_base = *tmem_slot;
 
-    if (warp == 0 || warp >= 22) {
-        // ===================== TMA producers: the other input's halo chunks =====================
-        const int prod = warp == 0 ? 0 : warp - 21;
-        if (prod < nprod) {
+    if (warp >= TC_CONSUMERS / 32) {
+        // ===================== TMA producer: the other input's halo chunks =====================
+        setmaxnreg_dec<40>();
+        if (warp == TC_CONSUMERS / 32 && lane == 0) {
             uint32_t bcount = 0;
             const uint64_t pol = l2_policy_evict_last();
-            auto load = [&](void *dst, const CUtensorMap *m, uint64_t *bar, int c0, int c1, int c2, int c3) {
-                if (hint) tma_load_4d_hint(dst, m, bar, c0, c1, c2, c3, pol);
-                else tma_load_4d(dst, m, bar, c0, c1, c2, c3);
-            };
             for (int g = t_begin + blockIdx.x; g < t_end; g += gridDim.x) {
                 const bool second = both ? (g & 1) : (g >= ntiles);
                 const TcTile T = tc_decode(both ? (g >> 1) : (second ? g - ntiles : g), nxt, nyt);
                 const int img = T.n * 4 + T.py * 2 + T.px;
                 const CUtensorMap *moh = second ? &m1h : &m2h, *mol = second ? &m1l : &m2l;
-                // one half-stage = the hi (then the lo) copy of a K-group's 48 halo positions x all C channels:
-                // ncb boxes of 6 KB on one barrier
                 for (int u = 0; u < TC_NU; ++u)
-                    for (int g = 0; g < TB_NG; ++g)
+                    for (int gr = 0; gr < TB_NG; ++gr)
                         for (int hl = 0; hl < 2; ++hl, ++bcount) {
-                            if ((int)(bcount % (uint32_t)nprod) != prod) continue;
-                            const int s = bcount % TB_NBST;
-                            mbar_wait(&b_empty[s], ((bcount / TB_NBST) & 1) ^ 1);
-                            if (elect_one_sync()) {
-                                mbar_arrive_expect_tx(&b_full[s], (uint32_t)(ncb * TB_GBLK));
-                                unsigned char *dst = sB + s * TB_BSTAGE;
-                                for (int j = 0; j < ncb; ++j)
-                                    load(dst + j * TB_GBLK, hl ? mol : moh, &b_full[s], j * TC_KB, T.xc0 - TC_DR + g * TB_GW,
-                                         T.yc0 - TC_DR + u * TC_UR, img);
-                            }
-                            __syncwarp();
+                            const int s = bcount % bst;
+                            mbar_wait(&b_empty[s], ((bcount / bst) & 1) ^ 1);
+                            mbar_arrive_expect_tx(&b_full[s], (uint32_t)(NKB * TB_GBLK));
+                            unsigned char *dst = sB + s * TB_BSTAGE;
+#pragma unroll
+                            for (int j = 0; j < NKB; ++j)
+                                tma_load_4d_hint(dst + j * TB_GBLK, hl ? mol : moh, &b_full[s], j * TC_KB,
+                                                 T.xc0 - TC_DR + gr * TB_GW, T.yc0 - TC_DR + u * TC_UR, img, pol);
                         }
             }
         }
-    } else if (warp == 1) {
-        // ===================== MMA issuer =====================
-        // The whole warp runs the control flow (converged); one elected lane issues the MMAs and
-        // commits.  (Issuing from `if (lane == 0)` made nvcc wrap every UTCHMMA in an
-        // ELECT / BRA.U.ANY per-active-lane loop: ~70 cycles per MMA, measured.)
+        return;
+    }
+    setmaxnreg_inc<232>();
+
+    const int wg = warp >> 2, wq = warp & 3;
+    // builder role: pixel bp of the warpgroup's 64 (a warp covers 4 tile rows x 8 pixels: its 32 two-byte stores of
+    // one (halo row, displacement) hit 32 different banks), halo rows {2 hp, 2 hp + 1}
+    const int hp = wq >> 1;
+    const int bp = (lane >> 3) * TC_TW + (wq & 1) * 8 + (lane & 7);
+    const int bpy = 4 * wg + (bp >> 4), bpx = bp & 15;
+    // accumulator fragment role: rows 16 wq + lane / 4 (+ 8) of the warpgroup
+    const int py_t = 4 * wg + wq, pxa = lane >> 2, q = lane & 3;
+    const int iplane = (int)plane;             // all tensors < 2^31 elements (checked by the C ABI)
+    unsigned char *aw = sA + wg * TB_NAST * TB_ASTG;
+    const float inv_nelems = 1.0f / (float)C;
+    uint32_t bcount = 0, ucount = 0;
+    for (int g = t_begin + blockIdx.x; g < t_end; g += gridDim.x) {
+        const bool second = both ? (g & 1) : (g >= ntiles);           // gradInput2 tile (block-uniform)
+        const TcTile T = tc_decode(both ? (g >> 1) : (second ? g - ntiles : g), nxt, nyt);
+        const int nbase = T.n * (TC_DS * TC_DS);
+        // Per-tile address set-up of the builder pixel (element offsets fit in 32 bits): for unit u the band row of
+        // halo row hrl = 2hp+hh starts at off[hh] + u * dstep; consecutive displacements are `step` apart.
+        int off[2], dstep, step, ystep, tj0[2], ys0[2];
+        uint32_t colmask = 0;                                  // displacements to load (gradInput2: source columns inside the image)
         {
-            const uint32_t idesc = umma_idesc_bf16_f32(128, C, 1, 1);   // N = C (<= 256), A and B MN-major
-            uint32_t bcount = 0, ucount = 0, tcount = 0;
-            for (int g = t_begin + blockIdx.x; g < t_end; g += gridDim.x, ++tcount) {
-                const int ab = tcount % TB_NACC;
-                mbar_wait(&acc_empty[ab], ((tcount / TB_NACC) & 1) ^ 1);
-                tcgen05_fence_after();
-                const uint32_t d = tmem_base + ab * 256;
-                for (int u = 0; u < TC_NU; ++u, ++ucount) {
-                    const int as = ucount % TB_NAST;
-                    const bool rec = dbg && blockIdx.x == 0 && ucount < 64 && lane == 0;
-                    if (rec) dbg[ucount * 8 + 4] = clock64();
-                    mbar_wait(&a_full[as], (ucount / TB_NAST) & 1);
-                    if (rec) dbg[ucount * 8 + 5] = clock64();
-                    tcgen05_fence_after();
-                    const uint32_t a_hi = smem_u32(sA + as * TB_ASTG), a_lo = a_hi + TB_AHL;
-                    long long bwait = 0;
-                    for (int g = 0; g < TB_NG; ++g)
-                        for (int hl = 0; hl < 2; ++hl, ++bcount) {
-                            const int s = bcount % TB_NBST;
-                            const long long tw0 = rec ? clock64() : 0;
-                            mbar_wait(&b_full[s], (bcount / TB_NBST) & 1);
-                            if (rec) bwait += clock64() - tw0;
-                            tcgen05_fence_after();
-                            if (elect_one_sync()) {
-                                const uint64_t bd = umma_desc_mn_sw128(smem_u32(sB + s * TB_BSTAGE), TB_GBLK);
-#pragma unroll
-                                for (int ks = 0; ks < TB_GK / 16; ++ks) {
-                                    const uint64_t ah = umma_desc_mn_sw128(a_hi + (g * TB_GK + ks * 16) * 128, TB_AMB);
-                                    const uint64_t kadv = (uint64_t)((ks * 16 * 128) >> 4);
-                                    if (hl == 0) {        // hi x hi, lo x hi
-                                        const uint64_t al = umma_desc_mn_sw128(a_lo + (g * TB_GK + ks * 16) * 128, TB_AMB);
-                                        umma_bf16_ss(d, ah, bd + kadv, idesc, (u | g | ks) != 0);
-                                        umma_bf16_ss(d, al, bd + kadv, idesc, 1);
-                                    } else {              // hi x lo
-                                        umma_bf16_ss(d, ah, bd + kadv, idesc, 1);
-                                    }
-                                }
-                                umma_commit(&b_empty[s]);
-                                if (g == TB_NG - 1 && hl == 1) umma_commit(&a_empty[as]);
-                            }
-                            __syncwarp();
-                        }
-                    if (rec) { dbg[ucount * 8 + 6] = clock64(); dbg[ucount * 8 + 7] = bwait; }
-                }
-                if (elect_one_sync()) umma_commit(&acc_full[ab]);
-                __syncwarp();
-            }
-        }
-    } else if (warp < 18) {
-        // ===================== builders: banded gradOutput matrix A (hi / lo) =====================
-        const int tb = tid - 64;                   // 0..511
-        // A warp covers 4 tile rows x 8 pixels: with the MN-major SW128 layout its 32 two-byte stores of
-        // one (halo row, displacement) hit 32 different banks (the K-major layout cost 6.5 wavefronts
-        // per store, ncu r1j), and its loads are 4 rows x 64 B.
-        const int sub = tb >> 7, wq = (tb >> 5) & 3;                          // sub-task; tile quadrant (warp-uniform)
-        const int p = ((wq >> 1) * 4 + (lane >> 3)) * TC_TW + (wq & 1) * 8 + (lane & 7);   // tile pixel
-        const int hp = sub >> 1, jh = sub & 1;     // halo rows {2hp, 2hp+1}; displacements [11*jh, 11*jh + nj)
-        const int j0 = jh * 11, nj = jh ? 10 : 11;
-        const int py_t = p >> 4, px_t = p & 15;
-        const int iplane = (int)plane;             // all tensors < 2^31 elements (checked by the C ABI)
-        // scatter offsets (unit-invariant): entry (hh, jj) -> k = (2hp+hh)*36 + px_t + j0 + jj
-        uint32_t offs[11];
-#pragma unroll
-        for (int jj = 0; jj < 11; ++jj) {
-            uint32_t two = 0;
-#pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-                const uint32_t k = tb_kindex(2 * hp + hh, px_t + j0 + jj);
-                two |= tb_a_offset(p, k) << (16 * hh);
-            }
-            offs[jj] = two;
-        }
-        uint32_t ucount = 0;
-        for (int g = t_begin + blockIdx.x; g < t_end; g += gridDim.x) {
-            const bool second = both ? (g & 1) : (g >= ntiles);           // gradInput2 tile (warp-uniform)
-            const TcTile T = tc_decode(both ? (g >> 1) : (second ? g - ntiles : g), nxt, nyt);
-            const int yc = T.yc0 + py_t, xc = T.xc0 + px_t;
+            const int yc = T.yc0 + bpy, xc = T.xc0 + bpx;
             const bool pix_ok = (yc < Hc) && (xc < Wc);
-            const int nbase = T.n * (TC_DS * TC_DS);
-            // Per-tile address set-up (element offsets fit in 32 bits): for unit u the band row of halo
-            // row hrl = 2hp+hh starts at off[hh] + u * dstep; consecutive displacements are `step` apart.
-            int off[2], dstep, step, ystep, tj0[2], ys0[2];
-            uint32_t colmask = 0;                                  // displacements to load (gradInput2: source columns inside the image)
 #pragma unroll
             for (int hh = 0; hh < 2; ++hh) {
                 const int hrl = 2 * hp + hh;
-                tj0[hh] = hrl - py_t;                              // tj + 10 at u = 0 (+4 per unit)
+                tj0[hh] = hrl - bpy;                               // tj + 10 at u = 0 (+4 per unit)
                 if (!second) {
                     ys0[hh] = pix_ok ? 0 : Hc;                     // gO at the output pixel itself
-                    off[hh] = ((nbase + tj0[hh] * TC_DS + j0) * H + (2 * yc + T.py)) * W + (2 * xc + T.px);
+                    off[hh] = ((nbase + tj0[hh] * TC_DS) * H + (2 * yc + T.py)) * W + (2 * xc + T.px);
                 } else {
                     ys0[hh] = T.yc0 - TC_DR + hrl;                 // source pixel row at u = 0 (+4 per unit)
-                    const int xs0 = T.xc0 - TC_DR + px_t + j0;     // source column for jj = 0
-                    off[hh] = ((nbase + (TC_DS - 1 - tj0[hh]) * TC_DS + (TC_DS - 1 - j0)) * H + (2 * ys0[hh] + T.py)) * W +
+                    const int xs0 = T.xc0 - TC_DR + bpx;           // source column for j = 0
+                    off[hh] = ((nbase + (TC_DS - 1 - tj0[hh]) * TC_DS + (TC_DS - 1)) * H + (2 * ys0[hh] + T.py)) * W +
                               (2 * xs0 + T.px);
                     if (hh == 0)
 #pragma unroll
-                        for (int jj = 0; jj < 11; ++jj)
-                            if ((unsigned)(xs0 + jj) < (unsigned)Wc) colmask |= 1u << jj;
+                        for (int j = 0; j < TC_DS; ++j)
+                            if ((unsigned)(xs0 + j) < (unsigned)Wc) colmask |= 1u << j;
                 }
             }
             if (!second) {
                 step = iplane;                                     // next ti -> next plane
                 dstep = TC_UR * TC_DS * iplane;                    // next unit -> tj + 4
                 ystep = 0;
-                colmask = (1u << nj) - 1u;
+                colmask = (1u << TC_DS) - 1u;
             } else {
                 ystep = TC_UR;
                 step = 2 - iplane;                                 // j -> j+1: -1 plane, +2 in x
                 dstep = -TC_UR * TC_DS * iplane + 2 * TC_UR * W;   // next unit: tj + 4 -> -84 planes; source row + 4 -> +8 rows
-                colmask &= (1u << nj) - 1u;
             }
-            // The 22 gradOutput values of a unit are loaded in two batches of 11 (halo rows 2hp and 2hp+1) that
-            // alternate with the two scatter halves: a batch is in flight while the other one is converted and
-            // stored.  (Issuing all 22 at once stalled 1.4-6 K cycles per unit on the L1 miss queue; spreading
-            // them moved that wait into the scatter phase -- same ~5.7 K cycles per unit, clock64 timeline: the
-            // builder is bound by the arrival rate of its half-used gradOutput sectors.)
-            auto load_half = [&](int hh, int u, float (&dst)[11]) {
+        }
+        float acc[C / 2];
+#pragma unroll
+        for (int i = 0; i < C / 2; ++i) acc[i] = 0.f;
+        wgmma_fence_operands(acc);
+        int prev = -1;                                         // ring slot read by the wgmma group in flight
+        for (int u = 0; u < TC_NU; ++u, ++ucount) {
+            // buffer ucount & 1 was last read by unit ucount - 2, complete since unit ucount - 1's first wait
+            unsigned char *ah = aw + (ucount & 1) * TB_ASTG, *al = ah + TB_AHL;
+#pragma unroll
+            for (int hh = 0; hh < 2; ++hh) {
                 const int tjp = tj0[hh] + u * TC_UR;
                 const bool row_ok = ((unsigned)tjp < (unsigned)TC_DS) && ((unsigned)(ys0[hh] + u * ystep) < (unsigned)Hc);
-                const int base = off[hh] + u * dstep;      // only dereferenced under `ok`
+                const int base = off[hh] + u * dstep;          // only dereferenced under `ok`
+                float v[TC_DS];
 #pragma unroll
-                for (int jj = 0; jj < 11; ++jj) {
-                    const bool ok = row_ok && ((colmask >> jj) & 1u);
-                    dst[jj] = ok ? __ldg(gout + (base + jj * step)) : 0.f;
+                for (int j = 0; j < TC_DS; ++j) {
+                    const bool ok = row_ok && ((colmask >> j) & 1u);
+                    v[j] = ok ? __ldg(gout + (base + j * step)) : 0.f;
                 }
-            };
-            auto scatter_half = [&](int hh, const float (&src)[11], unsigned char *ah, unsigned char *al) {
 #pragma unroll
-                for (int jj = 0; jj < 11; ++jj) {
-                    if (jj < nj) {
-                        const float x = src[jj];
-                        const __nv_bfloat16 h = __float2bfloat16_rn(x);
-                        const __nv_bfloat16 l = __float2bfloat16_rn(x - __bfloat162float(h));
-                        const uint32_t o = (offs[jj] >> (16 * hh)) & 0xFFFFu;
-                        *reinterpret_cast<unsigned short *>(ah + o) = __bfloat16_as_ushort(h);
-                        *reinterpret_cast<unsigned short *>(al + o) = __bfloat16_as_ushort(l);
+                for (int j = 0; j < TC_DS; ++j) {
+                    const __nv_bfloat16 h = __float2bfloat16_rn(v[j]);
+                    const __nv_bfloat16 l = __float2bfloat16_rn(v[j] - __bfloat162float(h));
+                    const uint32_t o = tb_a_offset(bp, tb_kindex(2 * hp + hh, bpx + j));   // unit-invariant
+                    *reinterpret_cast<unsigned short *>(ah + o) = __bfloat16_as_ushort(h);
+                    *reinterpret_cast<unsigned short *>(al + o) = __bfloat16_as_ushort(l);
+                }
+            }
+            fence_proxy_async();                               // generic-proxy writes -> visible to the tensor core
+            named_barrier_sync(1 + wg, 128);                   // the warpgroup's whole A is written
+            const uint32_t ah32 = smem_u32(ah), al32 = smem_u32(al);
+            for (int gr = 0; gr < TB_NG; ++gr)
+#pragma unroll
+                for (int hl = 0; hl < 2; ++hl, ++bcount) {
+                    const int s = bcount % bst;
+                    mbar_wait(&b_full[s], (bcount / bst) & 1);
+                    const uint32_t bb = smem_u32(sB + s * TB_BSTAGE);
+                    wgmma_fence();
+#pragma unroll
+                    for (int ks = 0; ks < TB_GK / 16; ++ks) {
+                        const uint32_t ko = (gr * TB_GK + ks * 16) * 128;
+                        const uint64_t bd = wgmma_desc_mn_sw128(bb + ks * 16 * 128, TB_GBLK);
+                        wgmma_bwd<NKB>(acc, wgmma_desc_mn_sw128(ah32 + ko, TB_AHL), bd);           // hi x hi | hi x lo
+                        if (hl == 0) wgmma_bwd<NKB>(acc, wgmma_desc_mn_sw128(al32 + ko, TB_AHL), bd);  // lo x hi
                     }
+                    wgmma_commit();
+                    wgmma_wait<1>();
+                    if (prev >= 0) mbar_arrive(&b_empty[prev]);
+                    prev = s;
                 }
-            };
-            float v0[11], v1[11];
-            load_half(0, 0, v0);
-            for (int u = 0; u < TC_NU; ++u, ++ucount) {
-                const int as = ucount % TB_NAST;
-                load_half(1, u, v1);
-                const bool rec = dbg && blockIdx.x == 0 && tb == 0 && ucount < 64;
-                if (rec) dbg[ucount * 8 + 0] = clock64();
-                mbar_wait(&a_empty[as], ((ucount / TB_NAST) & 1) ^ 1);
-                if (rec) dbg[ucount * 8 + 1] = clock64();
-                unsigned char *ah = sA + as * TB_ASTG, *al = ah + TB_AHL;
-                scatter_half(0, v0, ah, al);
-                if (u + 1 < TC_NU) load_half(0, u + 1, v0);
-                scatter_half(1, v1, ah, al);
-                fence_proxy_async();          // generic-proxy writes -> visible to the tensor core
-                if (rec) dbg[ucount * 8 + 2] = clock64();
-                __syncwarp();                 // every lane's stores + fence precede the warp's single arrival
-                if (lane == 0) mbar_arrive(&a_full[as]);
-                if (rec) dbg[ucount * 8 + 3] = clock64();
-            }
         }
-    } else {
-        // ===================== epilogue (warps 18..21) =====================
-        const int quad = warp & 3;
-        const int p = quad * 32 + lane;
-        const int py_t = p >> 4, px_t = p & 15;
-        const float inv_nelems = 1.0f / (float)C;
-        uint32_t tcount = 0;
-        for (int g = t_begin + blockIdx.x; g < t_end; g += gridDim.x, ++tcount) {
-            const bool second = both ? (g & 1) : (g >= ntiles);
-            const TcTile T = tc_decode(both ? (g >> 1) : (second ? g - ntiles : g), nxt, nyt);
-            const int yc = T.yc0 + py_t, xc = T.xc0 + px_t;
-            const bool pix_ok = (yc < Hc) && (xc < Wc);
-            float *o = (second ? gin2 : gin1) + (long)T.n * C * plane + (long)(2 * yc + T.py) * W + (2 * xc + T.px);
-            const int ab = tcount % TB_NACC;
-            mbar_wait(&acc_full[ab], (tcount / TB_NACC) & 1);
-            tcgen05_fence_after();
-            const uint32_t taddr = tmem_base + ((uint32_t)(quad * 32) << 16) + ab * 256;
-#pragma unroll 1
-            for (int c0 = 0; c0 < C; c0 += 32) {
-                float r[32];
-                tmem_ld16(taddr + c0, r);
-                tmem_ld16(taddr + c0 + 16, r + 16);
-                tmem_ld_wait();
-                if (pix_ok) {
+        wgmma_wait<0>();
+        wgmma_fence_operands(acc);
+        mbar_arrive(&b_empty[prev]);
+        // epilogue: fragment rows = tile pixels (py_t, pxa) and (py_t, pxa + 8), columns = channels
+        const int yc = T.yc0 + py_t, xc = T.xc0 + pxa;
+        const bool ok0 = (yc < Hc) && (xc < Wc), ok1 = (yc < Hc) && (xc + 8 < Wc);
+        float *o = (second ? gin2 : gin1) + (long)T.n * C * plane + (long)(2 * yc + T.py) * W + (2 * xc + T.px);
 #pragma unroll
-                    for (int i = 0; i < 32; ++i) __stcs(o + (long)(c0 + i) * plane, r[i] * inv_nelems);
-                }
-            }
-            tcgen05_fence_before();
-            mbar_arrive(&acc_empty[ab]);
-        }
+        for (int i = 0; i < C / 8; ++i)
+#pragma unroll
+            for (int j = 0; j < 4; ++j)
+                if ((j >> 1) ? ok1 : ok0)
+                    __stcs(o + 16 * (j >> 1) + (long)(8 * i + 2 * q + (j & 1)) * plane, acc[4 * i + j] * inv_nelems);
     }
-    tcgen05_fence_before();
-    __syncthreads();
-    if (warp == 1) tmem_dealloc<512>(tmem_base);
 }
 
 // ------------------------------------------------------------------------------------------------
 // Host side
 // ------------------------------------------------------------------------------------------------
-// tuning knobs for experiments (read per call, no cached state): FN2B200_TC_BST, FN2B200_TC_HINT
-static int tc_env_int(const char *name, int def, int lo, int hi) {
-    const char *e = getenv(name);
-    if (!e || !*e) return def;
-    int v = atoi(e);
-    return v < lo ? lo : (v > hi ? hi : v);
-}
-
 bool corr_tc_supported(const CorrParams &p) {
     return p.k == 1 && p.s1 == 1 && p.s2 == 2 && p.dr == TC_DR && p.pad == p.md && (p.H % 2 == 0) &&
            (p.W % 2 == 0) && (p.C % TC_KB == 0) && p.C <= TC_KB * TC_MAXKB && p.H >= 2 && p.W >= 2 &&
@@ -797,43 +570,35 @@ int corr_forward_tc(const float *in1, const float *in2, float *out, const CorrPa
     const int Hc = p.H / 2, Wc = p.W / 2;
     const int nxt = (Wc + TC_TW - 1) / TC_TW, nyt = (Hc + TC_TH - 1) / TC_TH;
     const int ntiles = p.B * 4 * nxt * nyt;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int nkb = p.C / TC_KB;
-    const int ts = tc_env_int("FN2B200_TC_TS", 1, 0, 1);       // A_hi from tensor memory (TS-mode MMAs); 0 = all operands from shared memory
     int bst = 2;
-    while (bst < TC_MAXBST && tc_smem_bytes(nkb, bst + 1, ts) <= TC_SMEM_MAX) ++bst;
-    bst = tc_env_int("FN2B200_TC_BST", bst, 2, bst);
-    const int hint = tc_env_int("FN2B200_TC_HINT", 1, 0, 1);
-    const int smem = tc_smem_bytes(nkb, bst, ts);
-    cudaError_t e = cudaFuncSetAttribute(corr_fwd_tc_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(corr_fwd_tc_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    while (bst < TC_MAXBST && tc_smem_bytes(nkb, bst + 1) <= TC_SMEM_MAX) ++bst;
+    const int smem = tc_smem_bytes(nkb, bst);
+    cudaError_t e = cudaFuncSetAttribute(corr_fwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return fail((int)e, "correlation_forward(tc): smem attribute (%s)", cudaGetErrorString(e));
     const int grid = ntiles < sms ? ntiles : sms;
-    // Producer-count rules (mbarrier parity waits only tell adjacent phases apart, so a producer must never be two
-    // phases ahead of the consumer on a barrier it did not itself visit one phase earlier):
-    //  * B slots: a producer's previous B stage is nprod stages back, so it is at most nprod + slots stages ahead
-    //    of the MMA warp -> nprod <= slots keeps it within one ring revolution;
-    //  * A blocks: with C = 256 a segment has 4 A jobs + 8 B jobs per unit; for nprod in {1, 2, 4} the job count of
-    //    every segment is a multiple of nprod, so each producer owns fixed A blocks and revisits the same a_empty
-    //    barrier every segment (safe by induction).  For C < 256 the A blocks would rotate between producers that
-    //    can be several short segments ahead (deep ring, few stages per segment): one producer there.
-    int np_max = 1;
-    if (nkb == TC_MAXKB)
-        while (2 * np_max <= TC_MAXPROD && 2 * np_max <= bst) np_max *= 2;
-    int nprod = tc_env_int("FN2B200_TC_NP", np_max, 1, np_max);
-    while (nprod & (nprod - 1)) --nprod;          // power of two
-    long long *dbg = nullptr;          // FN2B200_TC_DBG = device pointer: per-unit clock64 timeline of CTA 0 (tools/tc_timeline.py)
-    if (const char *ev = getenv("FN2B200_TC_DBG")) dbg = reinterpret_cast<long long *>(strtoull(ev, nullptr, 0));
-    if (ts)
-        corr_fwd_tc_kernel<true><<<grid, TC_THREADS, smem, st>>>(m1h, m1l, m2h, m2l, out, p.out_bstride, p.leaky, p.B, p.C, p.H,
-                                                                  p.W, ntiles, bst, hint, nprod, dbg);
-    else
-        corr_fwd_tc_kernel<false><<<grid, TC_THREADS, smem, st>>>(m1h, m1l, m2h, m2l, out, p.out_bstride, p.leaky, p.B, p.C, p.H,
-                                                                   p.W, ntiles, bst, hint, nprod, dbg);
+    corr_fwd_tc_kernel<<<grid, TC_THREADS, smem, st>>>(m1h, m1l, m2h, m2l, out, p.out_bstride, p.leaky, p.B, p.C, p.H, p.W,
+                                                       ntiles, bst);
     count_launch();
     return check_launch("correlation_forward(tc)");
+}
+
+template <int NKB>
+static int launch_bwd_tc_nkb(const CUtensorMap &m2h, const CUtensorMap &m2l, const CUtensorMap &m1h, const CUtensorMap &m1l,
+                             const float *gout, float *gin1, float *gin2, const CorrParams &p, int ntiles, int t_begin,
+                             int t_end, int grid, cudaStream_t st) {
+    int bst = 2;
+    while (bst < TB_MAXBST && tb_smem_bytes(bst + 1) <= TC_SMEM_MAX) ++bst;
+    const int smem = tb_smem_bytes(bst);
+    cudaError_t e = cudaFuncSetAttribute(corr_bwd_tc_kernel<NKB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) return fail((int)e, "correlation_backward(tc): smem attribute (%s)", cudaGetErrorString(e));
+    corr_bwd_tc_kernel<NKB><<<grid, TB_THREADS, smem, st>>>(m2h, m2l, m1h, m1l, gout, gin1, gin2, p.B, p.H, p.W, ntiles,
+                                                            t_begin, t_end, bst);
+    count_launch();
+    return check_launch("correlation_backward(tc)");
 }
 
 static int launch_bwd_tc(const __nv_bfloat16 *h1, const __nv_bfloat16 *l1, const __nv_bfloat16 *h2, const __nv_bfloat16 *l2,
@@ -849,24 +614,16 @@ static int launch_bwd_tc(const __nv_bfloat16 *h1, const __nv_bfloat16 *l1, const
     const int ntiles = p.B * 4 * nxt * nyt;
     const int t_begin = gin1 ? 0 : ntiles, t_end = gin2 ? 2 * ntiles : ntiles;
     if (t_end <= t_begin) return 0;
-    int dev = 0, sms = 148;
+    int dev = 0, sms = 132;
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    int bst = 2;
-    while (bst < TB_MAXBST && tb_smem_bytes(bst + 1) <= TC_SMEM_MAX) ++bst;
-    bst = tc_env_int("FN2B200_TC_BST", bst, 2, bst);
-    const int hint = tc_env_int("FN2B200_TC_HINT", 1, 0, 1);
-    const int smem = tb_smem_bytes(bst);
-    cudaError_t e = cudaFuncSetAttribute(corr_bwd_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) return fail((int)e, "correlation_backward(tc): smem attribute (%s)", cudaGetErrorString(e));
     const int grid = (t_end - t_begin) < sms ? (t_end - t_begin) : sms;
-    long long *dbg = nullptr;
-    if (const char *ev = getenv("FN2B200_TC_DBG")) dbg = reinterpret_cast<long long *>(strtoull(ev, nullptr, 0));
-    const int nprod = tc_env_int("FN2B200_TC_NP", TB_MAXPROD < bst ? TB_MAXPROD : bst, 1, TB_MAXPROD < bst ? TB_MAXPROD : bst);
-    corr_bwd_tc_kernel<<<grid, TB_THREADS, smem, st>>>(m2h, m2l, m1h, m1l, gout, gin1, gin2, p.B, p.C, p.H, p.W, ntiles, t_begin,
-                                                       t_end, bst, hint, nprod, dbg);
-    count_launch();
-    return check_launch("correlation_backward(tc)");
+    switch (p.C / TC_KB) {
+    case 1: return launch_bwd_tc_nkb<1>(m2h, m2l, m1h, m1l, gout, gin1, gin2, p, ntiles, t_begin, t_end, grid, st);
+    case 2: return launch_bwd_tc_nkb<2>(m2h, m2l, m1h, m1l, gout, gin1, gin2, p, ntiles, t_begin, t_end, grid, st);
+    case 3: return launch_bwd_tc_nkb<3>(m2h, m2l, m1h, m1l, gout, gin1, gin2, p, ntiles, t_begin, t_end, grid, st);
+    default: return launch_bwd_tc_nkb<4>(m2h, m2l, m1h, m1l, gout, gin1, gin2, p, ntiles, t_begin, t_end, grid, st);
+    }
 }
 
 // have_split != 0: the workspace already holds the hi/lo copies of (in1, in2) written by

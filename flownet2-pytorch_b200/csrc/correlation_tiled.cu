@@ -5,7 +5,7 @@
 //   channels_first x2 + correlation_backward_input1/2  (correlation_cuda_kernel.cu:150-241, :243-334,
 //                                                        launched once per sample, :519-554)
 //
-// B200 design (not a translation):
+// Design (not a translation):
 //   * No padded NHWC scratch copies and no memsets: TMA tensor maps over the ORIGINAL NCHW tensors,
 //     signed box coordinates + out-of-bounds zero fill give the zero padding for free.
 //   * One launch covers the whole batch (the reference loops over samples on the host in backward).

@@ -3,7 +3,7 @@
 // Replaces kernel_resample2d_update_output / _backward_input1 / _backward_input2
 // (reference resample2d_package/resample2d_kernel.cu:15-72, :75-125, :127-198).
 //
-// B200 design (HBM/L2-bound gather): ONE thread per output PIXEL (the reference uses one per
+// Design (HBM/L2-bound gather): ONE thread per output PIXEL (the reference uses one per
 // pixel x channel and re-reads the flow and recomputes taps per channel): the two flow values are
 // read once, tap indices / weights computed once, then the C channels are gathered with 4*C
 // independent loads in flight.  The image is addressed through explicit element strides so the

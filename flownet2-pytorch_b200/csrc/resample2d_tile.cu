@@ -10,11 +10,10 @@
 // at the L2->SM crossbar ceiling (0.51 GB moved for 0.117 GB of algorithmic traffic, 9.3 TB/s).  A CTA that owns a
 // 32 x (8 PY) pixel tile touches (32 + 2h) x (8 PY + 2h) pixels of the image instead: the sectors it pulls are reused
 // by its other threads out of L1 (the CTAs co-resident on an SM are x-neighbours and share their halos too).
-// Measured at cfg3 (profiles/r2/rs_sweep_v2_families.txt, ncu_resample_*.csv): L2->SM traffic 510 -> 120 MB, L1 hit rate
-// 86 %, forward 55.8 -> 48.9 us; what bounds it now is the L1 data pipe (4.7 wavefronts per warp-wide tap load, 70 % of its
-// peak).  Two alternatives were built, measured and dropped: a TMA-staged shared-memory box per CTA (same bytes, but flow
-// read -> box placement -> TMA -> gather serialise inside a CTA and 77 KB boxes leave 2 CTAs per SM: 49.8-73.9 us, 300 us
-// at sigma = 64) and, for the backward, accumulation in a shared-memory box (below).
+// What bounds it is the L1 data pipe (a warp-wide tap load touches many lines).  A TMA-staged shared-memory box per
+// CTA moves the same bytes, but flow read -> box placement -> TMA -> gather serialise inside a CTA and large boxes leave
+// few CTAs per SM; it was dropped, as was,
+// for the backward, accumulation in a shared-memory box (below).
 //
 // Thread (lx = tid & 31, ly = tid >> 5) owns pixels (tx0 + lx, ty0 + ly + 8 j), j < PY: flow reads and output stores
 // are 128-byte coalesced rows, the PY pixels give 4 C PY independent gathers in flight per thread.
@@ -112,15 +111,15 @@ resample2d_fwd_tile(ImgView im1, ImgView im0, FlowSrc fs, WarpOut o, int C, int 
 
 // ---------------------------------------------------------------------------------------------------------------
 // Backward.  One kernel: the flow gradient (K7, needs the image taps: gathered as in the forward) and the image
-// gradient (K6, a bilinear scatter of gradOutput).  What bounds the scatter (tools/atomics_bench.py, profiles/r2): an
-// SM retires global reductions at >= 1.2 cycles per LANE whatever their width, and round 1 issued 4 taps x C of them
-// per pixel (44 M at cfg3: 181 us for the scatter alone).  SC selects how the scatter is done:
+// gradient (K6, a bilinear scatter of gradOutput).  What bounds the scatter (csrc_test/atomics_bench.cu): an SM retires
+// global reductions at a fixed cost per LANE whatever their width, and round 1 issued 4 taps x C of them per pixel.
+// SC selects how the scatter is done:
 //   1  one red.global.add.f32 per tap and channel into the planar gradient (round 1; any shape)
 //   2  one red.global.add.v4.f32 per tap into a pixel-interleaved scratch T[b][y][x][4] (C <= 3), transposed into the
-//      planar gradient by resample2d_bwd_finish: 4 lane-operations per pixel instead of 12 (scatter alone 77 us)
+//      planar gradient by resample2d_bwd_finish: 4 lane-operations per pixel instead of 12
 // Accumulating in a shared-memory box per CTA and flushing it with coalesced vector reductions was built and measured
-// too: red.shared.add.f32 is a compare-and-swap loop on this architecture (ATOMS.CAST.SPIN) that retries whenever
-// neighbouring pixels hit the same word -- 175-210 us at sigma = 4 and 340-390 us on a smooth flow field: dropped.
+// too: red.shared.add.f32 compiled to a compare-and-swap loop that retries whenever neighbouring pixels hit the same
+// word, which made it slower than the global reductions: dropped.
 // ---------------------------------------------------------------------------------------------------------------
 template <int CT, int PY, int SC>
 __global__ void __launch_bounds__(256)

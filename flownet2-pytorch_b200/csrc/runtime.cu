@@ -7,7 +7,7 @@
 #include <string.h>
 
 #include "common.cuh"
-#include "umma.cuh"
+#include "wgmma.cuh"
 
 namespace fn2 {
 

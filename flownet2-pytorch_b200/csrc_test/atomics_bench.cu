@@ -1,5 +1,5 @@
 // atomics_bench.cu -- micro-benchmark of the reduction flavours a bilinear scatter (Resample2d backward) can be
-// built from.  Test / tuning hook only (tools/atomics_bench.py); lives in libfn2b200_test.so, not in the product.
+// built from.  Test / tuning hook only; lives in libfn2b200_test.so, not in the product.
 //
 // Every thread issues `iters` reductions to pseudo-random addresses inside a window of `window` floats that belongs
 // to its CTA (global modes: window placed at cta * window inside `buf`; shared modes: the CTA's shared memory).

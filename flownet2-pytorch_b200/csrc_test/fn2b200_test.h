@@ -1,7 +1,7 @@
 /*
  * fn2b200_test.h -- C ABI of libfn2b200_test.so: hardware self-tests and micro-benchmarks of the building blocks
- * (tcgen05 / TMEM / TMA descriptors, TMA feed rate, MMA issue rate, reduction flavours).  NOT part of the product:
- * libfn2b200.so neither contains nor links any of this; only tests/ and tools/ load this library.
+ * (wgmma / TMA descriptors, reduction flavours).  NOT part of the product:
+ * libfn2b200.so neither contains nor links any of this; only tests/ load this library.
  * Same conventions as include/fn2b200.h (device pointers, stream handle, 0 = success, thread-local error text).
  */
 #ifndef FN2B200_TEST_H_
@@ -15,32 +15,20 @@ const char *fn2b200_test_last_error(void);
 
 /* D[128 x 144] (fp32, row-major) = A[128 x K] * B[144 x K]^T; A, B bf16 row-major, K a positive multiple of 64.
  * Both operands from shared memory (K-major, 128-byte swizzle, loaded by TMA) -- the forward kernel's forms. */
-int fn2b200_test_umma_gemm_ss(const void *A_bf16, const void *B_bf16, float *D, int K, void *stream);
+int fn2b200_test_wgmma_gemm_ss(const void *A_bf16, const void *B_bf16, float *D, int K, void *stream);
 
-/* D[128 x 64] = A[128 x 144] * Bt[144 x 64]: A written to shared memory by the threads (a_sw32 = 0: no-swizzle
- * core-matrix layout, 1: 32-byte-swizzle K-major), Bt ([K][N] row-major) loaded as an MN-major SW128 operand --
- * the backward kernel's forms. */
-int fn2b200_test_umma_gemm_mn(const void *A_bf16, const void *Bt_bf16, float *D, int a_sw32, void *stream);
+/* D[128 x 64] = A[128 x 144] * Bt[144 x 64]: A written to shared memory by the threads, K-major (a_sw32 = 0: no-swizzle
+ * core-matrix layout, 1: 32-byte swizzle), Bt ([K][N] row-major) loaded as an MN-major SW128 operand -- the backward
+ * kernel's B form. */
+int fn2b200_test_wgmma_gemm_mn(const void *A_bf16, const void *Bt_bf16, float *D, int a_sw32, void *stream);
 
-/* The _ss product with A read from tensor memory (written there with tcgen05.st); K = 64, 128, 192 or 256. */
-int fn2b200_test_umma_gemm_ts(const void *A_bf16, const void *B_bf16, float *D, int K, void *stream);
+/* The _ss product with A taken from registers (wgmma's register-A form), the fragments read from global memory. */
+int fn2b200_test_wgmma_gemm_rs(const void *A_bf16, const void *B_bf16, float *D, int K, void *stream);
 
-/* The _ts product with A brought from shared memory (TMA, K-major SW128) into tensor memory by tcgen05.cp.128x256b. */
-int fn2b200_test_umma_gemm_tscp(const void *A_bf16, const void *B_bf16, float *D, int K, void *stream);
+/* The _rs product with A brought into shared memory by TMA (K-major SW128) and read from there into the fragments. */
+int fn2b200_test_wgmma_gemm_rs_tma(const void *A_bf16, const void *B_bf16, float *D, int K, void *stream);
 
-/* MMA issue-rate benchmark: D[sm] = cycles per M128 x N x K16 bf16 MMA on that SM (D holds >= #SM floats).
- * mode 0 = A, B from shared memory (K-major), 1 = A from tensor memory, 2 = A, B MN-major. */
-int fn2b200_test_umma_rate(float *D, int mode, int N, int iters, void *stream);
-
-/* TMA feed micro-benchmark (tools/tma_feed.py): persistent CTAs pull halo-style SW128 boxes (64 channels x box_w x
- * box_h) of a [nimg][Hc][Wc][C] bf16 tensor into a `stages`-deep ring with no consumer; out[2*cta] = cycles,
- * out[2*cta+1] = bytes.  cluster > 1: rank 0 issues every box with multicast (cluster < -1: every rank issues its
- * share); producer_warps (1..8, unicast only): that many warps each drive a private ring. */
-int fn2b200_test_tma_feed(const void *base_bf16, long long *out, int nimg, int C, int Hc, int Wc, int box_w, int box_h,
-                          int stages, int boxes_per_stage, int iters, int grid, int cluster, int producer_warps,
-                          void *stream);
-
-/* Reduction-flavour micro-benchmark (tools/atomics_bench.py, csrc_test/atomics_bench.cu): mode 0 red.global.f32,
+/* Reduction-flavour micro-benchmark (csrc_test/atomics_bench.cu): mode 0 red.global.f32,
  * 1 red.global.v2, 2 red.global.v4, 3 red.shared.f32, 4 plain shared RMW, 5 red.global.f32 with adjacent lane pairs.
  * buf holds grid * window floats (zeroed by the caller), cycles holds grid entries. */
 int fn2b200_test_atomics_bench(float *buf, long long *cycles, int mode, int window, int iters, int grid, void *stream);

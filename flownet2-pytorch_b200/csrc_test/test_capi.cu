@@ -3,13 +3,10 @@
 #include "fn2b200_test.h"
 
 namespace fn2 {
-int umma_selftest(const void *A, const void *B, float *D, int K, cudaStream_t st);
-int umma_selftest2(const void *A, const void *Bt, float *D, int a_sw32, cudaStream_t st);
-int umma_selftest_ts(const void *A, const void *B, float *D, int K, cudaStream_t st);
-int umma_selftest_tscp(const void *A, const void *B, float *D, int K, cudaStream_t st);
-int umma_rate_bench(float *out, int mode, int N, int iters, cudaStream_t st);
-int tma_feed_bench(const void *base, long long *out, int nimg, int C, int Hc, int Wc, int bw, int bh, int stages,
-                   int per_stage, int iters, int grid, int cluster, int warps, cudaStream_t st);
+int wgmma_selftest_ss(const void *A, const void *B, float *D, int K, cudaStream_t st);
+int wgmma_selftest_rs_global(const void *A, const void *B, float *D, int K, cudaStream_t st);
+int wgmma_selftest_rs_smem(const void *A, const void *B, float *D, int K, cudaStream_t st);
+int wgmma_selftest_mn(const void *A, const void *Bt, float *D, int a_sw32, cudaStream_t st);
 int atomics_bench(float *buf, long long *cycles, int mode, int window, int iters, int grid, cudaStream_t st);
 }  // namespace fn2
 using namespace fn2;
@@ -18,39 +15,27 @@ extern "C" {
 
 const char *fn2b200_test_last_error(void) { return last_error_text(); }
 
-int fn2b200_test_umma_gemm_ss(const void *A, const void *B, float *D, int K, void *stream) {
-    if (!A || !B || !D) return fail(FN2B200_ENULL, "test_umma_gemm_ss: null pointer");
+int fn2b200_test_wgmma_gemm_ss(const void *A, const void *B, float *D, int K, void *stream) {
+    if (!A || !B || !D) return fail(FN2B200_ENULL, "test_wgmma_gemm_ss: null pointer");
     if (int rc = bind_device_of(D)) return rc;
-    return umma_selftest(A, B, D, K, (cudaStream_t)stream);
+    return wgmma_selftest_ss(A, B, D, K, (cudaStream_t)stream);
 }
-int fn2b200_test_umma_gemm_mn(const void *A, const void *Bt, float *D, int a_sw32, void *stream) {
-    if (!A || !Bt || !D) return fail(FN2B200_ENULL, "test_umma_gemm_mn: null pointer");
+int fn2b200_test_wgmma_gemm_mn(const void *A, const void *Bt, float *D, int a_sw32, void *stream) {
+    if (!A || !Bt || !D) return fail(FN2B200_ENULL, "test_wgmma_gemm_mn: null pointer");
     if (int rc = bind_device_of(D)) return rc;
-    return umma_selftest2(A, Bt, D, a_sw32 != 0, (cudaStream_t)stream);
+    return wgmma_selftest_mn(A, Bt, D, a_sw32 != 0, (cudaStream_t)stream);
 }
-int fn2b200_test_umma_gemm_ts(const void *A, const void *B, float *D, int K, void *stream) {
-    if (!A || !B || !D) return fail(FN2B200_ENULL, "test_umma_gemm_ts: null pointer");
+int fn2b200_test_wgmma_gemm_rs(const void *A, const void *B, float *D, int K, void *stream) {
+    if (!A || !B || !D) return fail(FN2B200_ENULL, "test_wgmma_gemm_rs: null pointer");
     if (int rc = bind_device_of(D)) return rc;
-    return umma_selftest_ts(A, B, D, K, (cudaStream_t)stream);
+    return wgmma_selftest_rs_global(A, B, D, K, (cudaStream_t)stream);
 }
-int fn2b200_test_umma_gemm_tscp(const void *A, const void *B, float *D, int K, void *stream) {
-    if (!A || !B || !D) return fail(FN2B200_ENULL, "test_umma_gemm_tscp: null pointer");
+int fn2b200_test_wgmma_gemm_rs_tma(const void *A, const void *B, float *D, int K, void *stream) {
+    if (!A || !B || !D) return fail(FN2B200_ENULL, "test_wgmma_gemm_rs_tma: null pointer");
     if (int rc = bind_device_of(D)) return rc;
-    return umma_selftest_tscp(A, B, D, K, (cudaStream_t)stream);
+    return wgmma_selftest_rs_smem(A, B, D, K, (cudaStream_t)stream);
 }
-int fn2b200_test_umma_rate(float *D, int mode, int N, int iters, void *stream) {
-    if (!D) return fail(FN2B200_ENULL, "test_umma_rate: null pointer");
-    if (int rc = bind_device_of(D)) return rc;
-    return umma_rate_bench(D, mode, N, iters, (cudaStream_t)stream);
-}
-int fn2b200_test_tma_feed(const void *base_bf16, long long *out, int nimg, int C, int Hc, int Wc, int box_w, int box_h,
-                          int stages, int boxes_per_stage, int iters, int grid, int cluster, int producer_warps,
-                          void *stream) {
-    if (!base_bf16 || !out) return fail(FN2B200_ENULL, "test_tma_feed: null pointer");
-    if (int rc = bind_device_of(out)) return rc;
-    return tma_feed_bench(base_bf16, out, nimg, C, Hc, Wc, box_w, box_h, stages, boxes_per_stage, iters, grid, cluster,
-                          producer_warps, (cudaStream_t)stream);
-}
+
 int fn2b200_test_atomics_bench(float *buf, long long *cycles, int mode, int window, int iters, int grid, void *stream) {
     if (!buf || !cycles) return fail(FN2B200_ENULL, "test_atomics_bench: null pointer");
     if (int rc = bind_device_of(buf)) return rc;

@@ -2,7 +2,7 @@
 
 These are the functions the autograd wrappers and the ``*_cuda`` shim modules share.  PyTorch is
 used for allocation, the current device and the current stream only; all arithmetic happens in
-libfn2b200's hand-written sm_100a kernels.
+libfn2b200's hand-written sm_90a kernels.
 """
 import ctypes
 

@@ -3,8 +3,8 @@
 Pinned host memory is allocated on the NUMA node of the thread that calls ``cudaHostAlloc`` (first touch
 under that thread's CPU affinity / memory policy).  ``torchrun`` starts every rank without any affinity, so
 on a two-socket box half of the ranks stage their H2D / D2H traffic through the remote socket's memory
-controller and the inter-socket link -- round 1 measured the host-buffer (``e2e``) step going from 18.4 ms
-at 1 GPU to 37.7 ms at 8 GPUs for that reason while the kernels scaled perfectly.
+controller and the inter-socket link, which slows the host-buffer (``e2e``) step as ranks are added while the
+kernels scale perfectly.
 
 ``bind_to_device_node(dev)`` pins the calling process (CPU affinity + ``set_mempolicy(MPOL_PREFERRED)``)
 to the NUMA node the GPU's PCIe root port hangs off.  Call it BEFORE allocating pinned buffers.

@@ -46,7 +46,7 @@ def build(force=False):
     libdirs = ce.library_paths("cuda")
     # the system g++ (the one nvcc and torch's own extensions use), NOT $CXX: this image's $CXX is a private GCC whose
     # libstdc++ is static-only -- linked into an extension it brings a second, uninitialised copy of the iostream locale
-    # machinery and the first integer formatted into an error message segfaults (found on the B200 box)
+    # machinery and the first integer formatted into an error message segfaults
     cxx = os.environ.get("FN2B200_CXX", "g++")
 
     def one(name):

@@ -1,4 +1,4 @@
-"""Data-parallel sharding helpers -- the B200-native stand-in for the reference's
+"""Data-parallel sharding helpers -- the H100-native stand-in for the reference's
 ``nn.DataParallel`` wrapper (main.py:189,200: effective batch = batch_size x number_gpus).
 
 One process per GPU (``torchrun``); the three layers and the whole FlowNet2 forward are per-sample,

@@ -1,5 +1,5 @@
 /*
- * fn2b200.h -- C ABI of libfn2b200.so: B200 (sm_100a) kernels for flownet2-pytorch's three
+ * fn2b200.h -- C ABI of libfn2b200.so: H100 (sm_90a) kernels for flownet2-pytorch's three
  * custom layers.  This is the drop-in boundary: plain pointers and sizes, no torch types.
  *
  * Each entry point replaces one function of the reference's pybind extensions
@@ -72,7 +72,7 @@ int fn2b200_correlation_forward(const float *input1, const float *input2, float 
                                 int corr_type_multiply, void *stream);
 
 /*
- * Tensor-core forward (tcgen05, bf16 hi/lo operand split, fp32 accumulation in TMEM; error ~1e-5
+ * Tensor-core forward (wgmma, bf16 hi/lo operand split, fp32 accumulation in registers; error ~1e-5
  * relative, inside the 1e-4 contract).  It needs scratch for the split operands:
  * fn2b200_correlation_forward_workspace() returns the bytes required (0 = this configuration runs
  * on the FP32-FMA kernels; set the environment variable FN2B200_CORR_FWD=fma to force that), and
@@ -229,7 +229,7 @@ int fn2b200_channelnorm_backward_16(const void *input1, const void *output, cons
 /*
  * Introspection for benchmarks/tests: which kernel family the correlation entry points would
  * dispatch to for these parameters.  0 = generic gather kernels, 1 = TMA-tiled FP32-FMA kernels,
- * 2 = tensor cores (tcgen05) for forward AND backward when a workspace is supplied through the *_ws
+ * 2 = tensor cores (wgmma) for forward AND backward when a workspace is supplied through the *_ws
  * entry points (FN2B200_CORR_FWD=fma / FN2B200_CORR_BWD=fma select family 1 for that direction).
  */
 int fn2b200_correlation_path(int C, int H, int W, int pad_size, int kernel_size,

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Build recipe for ``oracle/_ref`` -- the REFERENCE's own CUDA kernels rebuilt for sm_100a.
+"""Build recipe for ``oracle/_ref`` -- the REFERENCE's own CUDA kernels rebuilt for sm_90a.
 
 TEST INFRASTRUCTURE ONLY.  Nothing under ``oracle/`` is on the product path; only ``tests/``,
 ``__graft_entry__.smoke()`` and ``bench.py``'s reference / cpu_baseline legs may load what this
@@ -13,7 +13,7 @@ What it does (needs ``/root/reference``; the GPU box only ever sees the prebuilt
    (SURVEY.md section 8c): drop ``-std=c++11`` and the sm_50..sm_70 ``-gencode`` list from each
    ``setup.py``; ``tensor.type()`` -> ``tensor.scalar_type()`` inside the ``AT_DISPATCH_*`` macros
    (correlation_cuda_kernel.cu:386,393,403,495,507,524,541; channelnorm_kernel.cu:111,152),
-3. builds each package with ``TORCH_CUDA_ARCH_LIST=10.0a`` and copies ONLY the resulting
+3. builds each package with ``TORCH_CUDA_ARCH_LIST=9.0a`` and copies ONLY the resulting
    ``*_cuda*.so`` files into ``oracle/_ref/`` (git-ignored, not gpurun-ignored),
 4. "installs" the reference's Python model code (models.py + networks/*.py, unmodified) into
    ``baseline/_ref/flownet2_pytorch/`` (git-ignored) so the end-to-end FlowNet2 / FlowNet2C
@@ -56,11 +56,11 @@ def build_extensions(force=False):
     if not os.path.isdir(REF):
         raise RuntimeError("reference tree %s not present and oracle/_ref is not prebuilt" % REF)
     work = tempfile.mkdtemp(prefix="fn2ref_")
-    env = dict(os.environ, TORCH_CUDA_ARCH_LIST="10.0a", MAX_JOBS=str(os.cpu_count() or 4))
+    env = dict(os.environ, TORCH_CUDA_ARCH_LIST="9.0a", MAX_JOBS=str(os.cpu_count() or 4))
     procs = []
     for p in PACKAGES:
         dst = os.path.join(work, p + "_package")
-        shutil.copytree(os.path.join(REF, "networks", p + "_package"), dst)
+        shutil.copytree(os.path.join(REF, "networks", p + "_package"), dst, copy_function=shutil.copyfile)   # writable copies
         _patch_setup(os.path.join(dst, "setup.py"))
         for f in os.listdir(dst):
             if f.endswith(".cu"):

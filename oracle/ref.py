@@ -1,4 +1,4 @@
-"""Loader for ``oracle/_ref`` -- the reference's own CUDA extensions rebuilt for sm_100a
+"""Loader for ``oracle/_ref`` -- the reference's own CUDA extensions rebuilt for sm_90a
 (TEST INFRASTRUCTURE ONLY; see oracle/build_ref.py).  Returns None when they are not built."""
 import glob
 import importlib.machinery

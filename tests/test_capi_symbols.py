@@ -27,14 +27,14 @@ def test_library_exports_every_declared_symbol():
     assert lib.fn2b200_version() == 100
 
 
-def test_library_is_sm100a_with_tma():
+def test_library_is_sm90a_with_tma():
     import subprocess
     import flownet2_b200
     try:
         out = subprocess.run(["cuobjdump", "-lelf", flownet2_b200._lib.LIB_PATH], capture_output=True, text=True).stdout
     except FileNotFoundError:
         pytest.skip("cuobjdump not available")
-    assert "sm_100a" in out
+    assert "sm_90a" in out
 
 
 def test_argument_validation_without_gpu():

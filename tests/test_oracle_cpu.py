@@ -3,7 +3,7 @@
 The reference ships no golden vectors (SURVEY section 4), so the restatement is pinned against
 (1) stock-PyTorch formulations + autograd in fp64 (tests/torch_ref.py), (2) hand-derived
 known-answer cases (SURVEY 8c), and (3) committed outputs of the reference's OWN kernels rebuilt for
-sm_100a and run on a B200 (tests/golden/*.npz, produced by tests/golden/make_golden.py).
+sm_90a and run on an H100 (tests/golden/*.npz, produced by tests/golden/make_golden.py).
 """
 import glob
 import os
@@ -128,12 +128,13 @@ def test_channelnorm_known_answers_and_torch():
     assert_close(orc.channelnorm_backward(t.detach().numpy(), o, go.numpy()), t.grad.numpy(), 1e-6, "oracle cnorm bwd")
 
 
-GOLDEN = sorted(glob.glob(os.path.join(os.path.dirname(__file__), "golden", "*.npz")))
+GOLDEN = sorted(p for p in glob.glob(os.path.join(os.path.dirname(__file__), "golden", "*.npz"))
+                if not os.path.basename(p).startswith("refk_"))   # refk_*: test_gpu_parity's reference-kernel results
 
 
 @pytest.mark.parametrize("path", GOLDEN or [None])
 def test_oracle_matches_reference_kernel_golden(path):
-    """Fixtures = outputs of the REFERENCE kernels (oracle/_ref, rebuilt for sm_100a) run on a B200."""
+    """Fixtures = outputs of the REFERENCE kernels (oracle/_ref, rebuilt for sm_90a) run on an H100."""
     if path is None:
         pytest.skip("no golden fixtures committed yet (generate with tests/golden/make_golden.py on a GPU box)")
     z = np.load(path)

@@ -1,5 +1,5 @@
-"""ctypes binding of libfn2b200_test.so (flownet2-pytorch_b200/csrc_test/fn2b200_test.h): hardware self-tests and
-micro-benchmarks.  Only tests/ and tools/ load it -- the product package never does."""
+"""ctypes binding of libfn2b200_test.so (flownet2-pytorch_b200/csrc_test/fn2b200_test.h): hardware self-tests
+and micro-benchmarks.  Only tests/ load it -- the product package never does."""
 import ctypes
 import os
 
@@ -7,8 +7,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB_PATH = os.path.join(ROOT, "flownet2-pytorch_b200", "libfn2b200_test.so")
 HEADER = os.path.join(ROOT, "flownet2-pytorch_b200", "csrc_test", "fn2b200_test.h")
 
-SYMBOLS = ("fn2b200_test_last_error", "fn2b200_test_umma_gemm_ss", "fn2b200_test_umma_gemm_mn", "fn2b200_test_umma_gemm_ts",
-           "fn2b200_test_umma_gemm_tscp", "fn2b200_test_umma_rate", "fn2b200_test_tma_feed", "fn2b200_test_atomics_bench")
+SYMBOLS = ("fn2b200_test_last_error", "fn2b200_test_wgmma_gemm_ss", "fn2b200_test_wgmma_gemm_mn", "fn2b200_test_wgmma_gemm_rs",
+           "fn2b200_test_wgmma_gemm_rs_tma", "fn2b200_test_atomics_bench")
 
 
 def load():
@@ -17,12 +17,8 @@ def load():
     lib = ctypes.CDLL(LIB_PATH)
     p, i = ctypes.c_void_p, ctypes.c_int
     lib.fn2b200_test_last_error.restype = ctypes.c_char_p
-    lib.fn2b200_test_umma_gemm_ss.argtypes = [p, p, p, i, p]
-    lib.fn2b200_test_umma_gemm_mn.argtypes = [p, p, p, i, p]
-    lib.fn2b200_test_umma_gemm_ts.argtypes = [p, p, p, i, p]
-    lib.fn2b200_test_umma_gemm_tscp.argtypes = [p, p, p, i, p]
-    lib.fn2b200_test_umma_rate.argtypes = [p, i, i, i, p]
-    lib.fn2b200_test_tma_feed.argtypes = [p, p] + [i] * 12 + [p]
+    for s in SYMBOLS[1:5]:
+        getattr(lib, s).argtypes = [p, p, p, i, p]
     lib.fn2b200_test_atomics_bench.argtypes = [p, p, i, i, i, i, p]
     for s in SYMBOLS[1:]:
         getattr(lib, s).restype = i
