@@ -51,6 +51,9 @@ def _load():
     lib.fn2b200_correlation_backward_workspace.restype = ctypes.c_size_t
     lib.fn2b200_correlation_backward_ws.argtypes = ([_c_ptr] * 5 + [_c_int] * 10 + [_c_ptr, ctypes.c_size_t, _c_int, _c_ptr])
     lib.fn2b200_correlation_backward_ws.restype = _c_int
+    lib.fn2b200_correlation_backward_cat.argtypes = ([_c_ptr] * 4 + [_c_int, _c_int, ctypes.c_float] + [_c_ptr] * 2
+                                                     + [_c_int] * 10 + [_c_ptr, ctypes.c_size_t, _c_int, _c_ptr])
+    lib.fn2b200_correlation_backward_cat.restype = _c_int
     lib.fn2b200_resample2d_forward.argtypes = [_c_ptr, lp, _c_ptr, _c_ptr] + [_c_int] * 8 + [_c_ptr]
     lib.fn2b200_resample2d_forward_up.argtypes = [_c_ptr, lp, _c_ptr, _c_int, _c_int, _c_int, ctypes.c_float, _c_ptr] + [_c_int] * 4 + [_c_ptr]
     lib.fn2b200_resample2d_forward_up.restype = _c_int
@@ -89,7 +92,7 @@ SYMBOLS = (
     "fn2b200_correlation_out_shape", "fn2b200_correlation_path",
     "fn2b200_correlation_forward", "fn2b200_correlation_backward",
     "fn2b200_correlation_forward_workspace", "fn2b200_correlation_forward_ws", "fn2b200_correlation_forward_cat",
-    "fn2b200_correlation_backward_workspace", "fn2b200_correlation_backward_ws",
+    "fn2b200_correlation_backward_workspace", "fn2b200_correlation_backward_ws", "fn2b200_correlation_backward_cat",
     "fn2b200_resample2d_forward", "fn2b200_resample2d_backward",
     "fn2b200_resample2d_forward_up", "fn2b200_warp_concat_forward",
     "fn2b200_warp_concat_backward_workspace", "fn2b200_warp_concat_backward",

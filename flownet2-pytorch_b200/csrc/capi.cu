@@ -32,6 +32,8 @@ static int fill_corr_params(CorrParams &p, int B, int C, int H, int W, int pad, 
         return fail(FN2B200_EINVAL, "correlation: tensor exceeds 2^31 elements");
     p.out_bstride = (long)p.D * p.oH * p.oW;
     p.leaky = 1.f;
+    p.g_bstride = p.out_bstride;
+    p.act = nullptr;
     return 0;
 }
 
@@ -203,6 +205,42 @@ int fn2b200_correlation_backward_ws(const float *in1, const float *in2, const fl
     }
     return fn2b200_correlation_backward(in1, in2, gout, gin1, gin2, B, C, H, W, pad, k, md, s1, s2,
                                         corr_type_multiply, stream);
+}
+
+int fn2b200_correlation_backward_cat(const float *in1, const float *in2, const float *grad_cat, const float *cat,
+                                     int cat_channels, int ch_offset, float leaky_slope, float *gin1, float *gin2, int B,
+                                     int C, int H, int W, int pad, int k, int md, int s1, int s2, int corr_type_multiply,
+                                     void *workspace, size_t workspace_bytes, int workspace_has_split, void *stream) {
+    (void)corr_type_multiply;
+    CorrParams p;
+    int rc = fill_corr_params(p, B, C, H, W, pad, k, md, s1, s2);
+    if (rc) return rc;
+    if (!(leaky_slope >= 0.f))
+        return fail(FN2B200_EINVAL, "correlation_backward_cat: leaky_slope %g < 0 (the sign of the activated output no "
+                    "longer tells which side of 0 the correlation was on)", (double)leaky_slope);
+    if (ch_offset < 0 || cat_channels < ch_offset + p.D)
+        return fail(FN2B200_EINVAL, "correlation_backward_cat: channels [%d, %d) do not fit a %d-channel buffer", ch_offset,
+                    ch_offset + p.D, cat_channels);
+    if ((int64_t)B * cat_channels * p.oH * p.oW >= (1LL << 31))
+        return fail(FN2B200_EINVAL, "correlation_backward_cat: tensor exceeds 2^31 elements");
+    if (s1 != 1)
+        return fail(FN2B200_EUNSUPPORTED, "correlation_backward_cat: stride1=%d unsupported (as fn2b200_correlation_backward)",
+                    s1);
+    if (B == 0) return 0;
+    const bool act = leaky_slope != 1.f;
+    if (!in1 || !in2 || !grad_cat || (act && !cat)) return fail(FN2B200_ENULL, "correlation_backward_cat: null pointer");
+    if (!gin1 && !gin2) return 0;
+    const long plane = (long)p.oH * p.oW;
+    const float *gout = grad_cat + ch_offset * plane;
+    p.g_bstride = cat_channels * plane;
+    p.act = act ? cat + ch_offset * plane : nullptr;
+    p.leaky = leaky_slope;
+    if ((rc = bind_device_of(in1))) return rc;
+    cudaStream_t st = (cudaStream_t)stream;
+    if (workspace && tc_bwd_enabled() && corr_tc_supported(p) && workspace_bytes >= corr_tc_workspace_bytes(p))
+        return corr_backward_tc(in1, in2, gout, gin1, gin2, p, workspace, workspace_bytes, workspace_has_split, st);
+    if (corr_tiled_supported(p)) return corr_backward_tiled(in1, in2, gout, gin1, gin2, p, st);
+    return corr_backward_generic(in1, in2, gout, gin1, gin2, p, st);
 }
 
 // shared argument checks of the fused warp-concat entry points

@@ -180,6 +180,11 @@ struct CorrParams {
     // concat buffer), and v < 0 is multiplied by `leaky` (1 = no activation, 0.1 = nn.LeakyReLU(0.1)).
     long out_bstride;
     float leaky;
+    // backward input placement / activation (fn2b200_correlation_backward_cat): sample n's D gradOutput planes start at
+    // gout + n * g_bstride (D*oH*oW = dense; larger = a channel range of a concat gradient).  act != NULL: the forward's
+    // activated output, same layout as gout; every gradOutput value g becomes (act > 0 ? g : g * leaky) before use.
+    long g_bstride;
+    const float *act;
 };
 int corr_forward_generic(const float *in1, const float *in2, float *out, const CorrParams &p,
                          cudaStream_t st);

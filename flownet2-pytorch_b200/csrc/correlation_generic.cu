@@ -72,7 +72,8 @@ corr_bwd_generic_kernel(const float *__restrict__ other, const float *__restrict
     int y = by + p.pad, x = bx + p.pad;
     const long hw = (long)p.H * p.W, ohw = (long)p.oH * p.oW;
     const float *src = other + ((long)n * p.C + c) * hw;
-    const float *g = gout + (long)n * p.D * ohw;
+    const float *g = gout + (long)n * p.g_bstride;
+    const float *ga = p.act ? p.act + (long)n * p.g_bstride : nullptr;
     float acc = 0.f;
     for (int tc = 0; tc < p.D; ++tc) {
         int i2 = (tc % p.ds - p.dr) * p.s2, j2 = (tc / p.ds - p.dr) * p.s2;
@@ -94,7 +95,13 @@ corr_bwd_generic_kernel(const float *__restrict__ other, const float *__restrict
         float w = 0.f;
         const float *gp = g + (long)tc * ohw;
         for (int j = ymin; j <= ymax; ++j)
-            for (int i = xmin; i <= xmax; ++i) w += __ldg(gp + (long)j * p.oW + i);
+            for (int i = xmin; i <= xmax; ++i) {
+                const long o = (long)j * p.oW + i;
+                float gv = __ldg(gp + o);
+                // LeakyReLU's derivative per element, before the window sum (bit-identical to masking in torch first)
+                if (ga) gv = __ldg(ga + (long)tc * ohw + o) > 0.f ? gv : gv * p.leaky;
+                w += gv;
+            }
         acc += w * v;
     }
     gin[idx] = acc / (float)(p.k * p.k * p.C);

@@ -335,11 +335,15 @@ template <> __device__ __forceinline__ void wgmma_bwd<4>(float (&d)[128], uint64
 // Both gradients in ONE launch: global tiles [t_begin, t_end) of [0, 2 ntiles).  One gradient only: tile g < ntiles
 // is tile g of gradInput1 (B = input2's halo, maps m2h / m2l), tile g >= ntiles is tile g - ntiles of gradInput2
 // (B = input1's halo); both: g = 2 tile + (0 = gradInput1, 1 = gradInput2).
-template <int NKB>
+// CAT (fn2b200_correlation_backward_cat): sample n's gradOutput planes start at gout + n * gplanes planes (a channel
+// range of a concat gradient), and with act != NULL every gradOutput value g is replaced by (act > 0 ? g : g * slope),
+// act read at g's offset, before the bf16 split.  !CAT: gplanes = 441, no activation (act, slope unused).
+template <int NKB, bool CAT>
 __global__ void __launch_bounds__(TB_THREADS, 1)
 corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constant__ CUtensorMap m2l,
                    const __grid_constant__ CUtensorMap m1h, const __grid_constant__ CUtensorMap m1l,
-                   const float *__restrict__ gout, float *__restrict__ gin1, float *__restrict__ gin2, int B,
+                   const float *__restrict__ gout, const float *__restrict__ act, int gplanes, float slope,
+                   float *__restrict__ gin1, float *__restrict__ gin2, int B,
                    int H, int W, int ntiles, int t_begin, int t_end, int bst) {
     constexpr int C = NKB * TC_KB;
     extern __shared__ __align__(1024) unsigned char smem_raw[];
@@ -412,7 +416,7 @@ corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constan
     for (int g = t_begin + blockIdx.x; g < t_end; g += gridDim.x) {
         const bool second = both ? (g & 1) : (g >= ntiles);           // gradInput2 tile (block-uniform)
         const TcTile T = tc_decode(both ? (g >> 1) : (second ? g - ntiles : g), nxt, nyt);
-        const int nbase = T.n * (TC_DS * TC_DS);
+        const int nbase = T.n * (CAT ? gplanes : TC_DS * TC_DS);
         // Per-tile address set-up of the builder pixel (element offsets fit in 32 bits): for unit u the band row of
         // halo row hrl = 2hp+hh starts at off[hh] + u * dstep; consecutive displacements are `step` apart.
         int off[2], dstep, step, ystep, tj0[2], ys0[2];
@@ -462,11 +466,26 @@ corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constan
                 const int tjp = tj0[hh] + u * TC_UR;
                 const bool row_ok = ((unsigned)tjp < (unsigned)TC_DS) && ((unsigned)(ys0[hh] + u * ystep) < (unsigned)Hc);
                 const int base = off[hh] + u * dstep;          // only dereferenced under `ok`
+                // CAT with activation: the activations are reduced to a bit per displacement (act > 0) before the
+                // gradOutput loads, so that 21 values, not 42, are in flight next to the 128-register accumulator
+                uint32_t pos = ~0u;
+                if (CAT && act) {
+                    float a[TC_DS];
+#pragma unroll
+                    for (int j = 0; j < TC_DS; ++j) {           // predicated, not branched: all 21 loads in flight
+                        const bool ok = row_ok && ((colmask >> j) & 1u);
+                        a[j] = ok ? __ldg(act + (base + j * step)) : 1.f;
+                    }
+                    pos = 0u;
+#pragma unroll
+                    for (int j = 0; j < TC_DS; ++j) pos |= a[j] > 0.f ? 1u << j : 0u;
+                }
                 float v[TC_DS];
 #pragma unroll
                 for (int j = 0; j < TC_DS; ++j) {
                     const bool ok = row_ok && ((colmask >> j) & 1u);
                     v[j] = ok ? __ldg(gout + (base + j * step)) : 0.f;
+                    if (CAT) v[j] = ((pos >> j) & 1u) ? v[j] : v[j] * slope;
                 }
 #pragma unroll
                 for (int j = 0; j < TC_DS; ++j) {
@@ -586,19 +605,33 @@ int corr_forward_tc(const float *in1, const float *in2, float *out, const CorrPa
     return check_launch("correlation_forward(tc)");
 }
 
-template <int NKB>
+template <int NKB, bool CAT>
 static int launch_bwd_tc_nkb(const CUtensorMap &m2h, const CUtensorMap &m2l, const CUtensorMap &m1h, const CUtensorMap &m1l,
                              const float *gout, float *gin1, float *gin2, const CorrParams &p, int ntiles, int t_begin,
                              int t_end, int grid, cudaStream_t st) {
     int bst = 2;
     while (bst < TB_MAXBST && tb_smem_bytes(bst + 1) <= TC_SMEM_MAX) ++bst;
     const int smem = tb_smem_bytes(bst);
-    cudaError_t e = cudaFuncSetAttribute(corr_bwd_tc_kernel<NKB>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    cudaError_t e = cudaFuncSetAttribute(corr_bwd_tc_kernel<NKB, CAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
     if (e != cudaSuccess) return fail((int)e, "correlation_backward(tc): smem attribute (%s)", cudaGetErrorString(e));
-    corr_bwd_tc_kernel<NKB><<<grid, TB_THREADS, smem, st>>>(m2h, m2l, m1h, m1l, gout, gin1, gin2, p.B, p.H, p.W, ntiles,
-                                                            t_begin, t_end, bst);
+    // gradOutput planes per sample: the 2^31-element check on the gradient buffer keeps every offset in 32 bits
+    const int gplanes = (int)(p.g_bstride / ((long)p.oH * p.oW));
+    corr_bwd_tc_kernel<NKB, CAT><<<grid, TB_THREADS, smem, st>>>(m2h, m2l, m1h, m1l, gout, p.act, gplanes, p.leaky, gin1,
+                                                                 gin2, p.B, p.H, p.W, ntiles, t_begin, t_end, bst);
     count_launch();
     return check_launch("correlation_backward(tc)");
+}
+
+template <bool CAT>
+static int launch_bwd_tc_c(const CUtensorMap &m2h, const CUtensorMap &m2l, const CUtensorMap &m1h, const CUtensorMap &m1l,
+                           const float *gout, float *gin1, float *gin2, const CorrParams &p, int ntiles, int t_begin,
+                           int t_end, int grid, cudaStream_t st) {
+    switch (p.C / TC_KB) {
+    case 1: return launch_bwd_tc_nkb<1, CAT>(m2h, m2l, m1h, m1l, gout, gin1, gin2, p, ntiles, t_begin, t_end, grid, st);
+    case 2: return launch_bwd_tc_nkb<2, CAT>(m2h, m2l, m1h, m1l, gout, gin1, gin2, p, ntiles, t_begin, t_end, grid, st);
+    case 3: return launch_bwd_tc_nkb<3, CAT>(m2h, m2l, m1h, m1l, gout, gin1, gin2, p, ntiles, t_begin, t_end, grid, st);
+    default: return launch_bwd_tc_nkb<4, CAT>(m2h, m2l, m1h, m1l, gout, gin1, gin2, p, ntiles, t_begin, t_end, grid, st);
+    }
 }
 
 static int launch_bwd_tc(const __nv_bfloat16 *h1, const __nv_bfloat16 *l1, const __nv_bfloat16 *h2, const __nv_bfloat16 *l2,
@@ -618,12 +651,10 @@ static int launch_bwd_tc(const __nv_bfloat16 *h1, const __nv_bfloat16 *l1, const
     cudaGetDevice(&dev);
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     const int grid = (t_end - t_begin) < sms ? (t_end - t_begin) : sms;
-    switch (p.C / TC_KB) {
-    case 1: return launch_bwd_tc_nkb<1>(m2h, m2l, m1h, m1l, gout, gin1, gin2, p, ntiles, t_begin, t_end, grid, st);
-    case 2: return launch_bwd_tc_nkb<2>(m2h, m2l, m1h, m1l, gout, gin1, gin2, p, ntiles, t_begin, t_end, grid, st);
-    case 3: return launch_bwd_tc_nkb<3>(m2h, m2l, m1h, m1l, gout, gin1, gin2, p, ntiles, t_begin, t_end, grid, st);
-    default: return launch_bwd_tc_nkb<4>(m2h, m2l, m1h, m1l, gout, gin1, gin2, p, ntiles, t_begin, t_end, grid, st);
-    }
+    // the dense, activation-free gradient of fn2b200_correlation_backward keeps the original instantiations
+    if (p.act || p.g_bstride != (long)p.D * p.oH * p.oW)
+        return launch_bwd_tc_c<true>(m2h, m2l, m1h, m1l, gout, gin1, gin2, p, ntiles, t_begin, t_end, grid, st);
+    return launch_bwd_tc_c<false>(m2h, m2l, m1h, m1l, gout, gin1, gin2, p, ntiles, t_begin, t_end, grid, st);
 }
 
 // have_split != 0: the workspace already holds the hi/lo copies of (in1, in2) written by

@@ -181,9 +181,11 @@ corr_fwd_tiled_kernel(const __grid_constant__ CUtensorMap map1,
 }
 
 // ------------------------------------------------------------------------------------------------
-// Backward (WHICH == 1: gradInput1 from input2; WHICH == 2: gradInput2 from input1)
+// Backward (WHICH == 1: gradInput1 from input2; WHICH == 2: gradInput2 from input1).
+// ACT: each stage also holds the forward's activated output at the gradOutput box's coordinates, and every gradOutput
+// value g becomes (act > 0 ? g : g * p.leaky) as it moves to registers (fn2b200_correlation_backward_cat).
 // ------------------------------------------------------------------------------------------------
-template <int S2, int DR, int WHICH>
+template <int S2, int DR, int WHICH, bool ACT = false>
 struct BwdCfg {
     static constexpr int DS = 2 * DR + 1;
     static constexpr int CB = 64;                                  // channels per CTA
@@ -196,17 +198,38 @@ struct BwdCfg {
     static constexpr int GW = (WHICH == 1) ? kTW : FW0;            // gradOutput row width staged
     static constexpr int F_STAGE = CB * FW;                        // floats
     static constexpr int G_STAGE = round_up(DS * GW, 32);          // floats (128-B multiple)
-    static constexpr int STAGE = F_STAGE + G_STAGE;
-    static constexpr uint32_t STAGE_BYTES = (CB * FW + DS * GW) * 4u;
+    static constexpr int NG = ACT ? 2 : 1;                          // gradOutput (+ activation) boxes per stage
+    static constexpr int STAGE = F_STAGE + NG * G_STAGE;
+    static constexpr uint32_t STAGE_BYTES = (CB * FW + NG * DS * GW) * 4u;
     static constexpr size_t SMEM = (size_t)kNST * STAGE * 4 + 128 + kNST * 8;
 };
 
-template <int S2, int DR, int WHICH>
+// 8 consecutive floats from shared memory; `sh` = the row's word offset, a compile-time constant after unrolling,
+// picks the widest aligned access
+__device__ __forceinline__ void lds_row8(const float *q, int sh, float *d) {
+    if ((sh & 3) == 0) {
+        float4 v0 = *reinterpret_cast<const float4 *>(q);
+        float4 v1 = *reinterpret_cast<const float4 *>(q + 4);
+        d[0] = v0.x; d[1] = v0.y; d[2] = v0.z; d[3] = v0.w;
+        d[4] = v1.x; d[5] = v1.y; d[6] = v1.z; d[7] = v1.w;
+    } else if ((sh & 1) == 0) {
+#pragma unroll
+        for (int h = 0; h < 4; ++h) {
+            float2 v = *reinterpret_cast<const float2 *>(q + 2 * h);
+            d[2 * h] = v.x; d[2 * h + 1] = v.y;
+        }
+    } else {
+#pragma unroll
+        for (int i = 0; i < kPX; ++i) d[i] = q[i];
+    }
+}
+
+template <int S2, int DR, int WHICH, bool ACT>
 __global__ void __launch_bounds__(256, 1)
 corr_bwd_tiled_kernel(const __grid_constant__ CUtensorMap map_other,
-                      const __grid_constant__ CUtensorMap map_g, float *__restrict__ gin,
-                      CorrParams p) {
-    using Cfg = BwdCfg<S2, DR, WHICH>;
+                      const __grid_constant__ CUtensorMap map_g, const __grid_constant__ CUtensorMap map_a,
+                      float *__restrict__ gin, CorrParams p) {
+    using Cfg = BwdCfg<S2, DR, WHICH, ACT>;
     constexpr int DS = Cfg::DS, CB = Cfg::CB, CC = Cfg::CC;
     constexpr int HALO = Cfg::HALO, WINP = Cfg::WINP, FW = Cfg::FW, GW = Cfg::GW;
     constexpr int SGN = (WHICH == 1) ? 1 : -1;
@@ -228,6 +251,7 @@ corr_bwd_tiled_kernel(const __grid_constant__ CUtensorMap map_other,
     if (tid == 0) {
         prefetch_tensormap(&map_other);
         prefetch_tensormap(&map_g);
+        if (ACT) prefetch_tensormap(&map_a);
         for (int i = 0; i < kNST; ++i) mbar_init(&full[i], 1);
         fence_barrier_init();
     }
@@ -241,10 +265,13 @@ corr_bwd_tiled_kernel(const __grid_constant__ CUtensorMap map_other,
         float *gs = fs + Cfg::F_STAGE;
         mbar_arrive_expect_tx(&full[st], Cfg::STAGE_BYTES);
         tma_load_4d(fs, &map_other, &full[st], x0 - HALO, y + SGN * tj * S2, c0, n);
-        if (WHICH == 1)
+        if (WHICH == 1) {
             tma_load_4d(gs, &map_g, &full[st], x0 - off, y - off, t * DS, n);
-        else
+            if (ACT) tma_load_4d(gs + Cfg::G_STAGE, &map_a, &full[st], x0 - off, y - off, t * DS, n);
+        } else {
             tma_load_4d(gs, &map_g, &full[st], x0 - off - HALO, y - tj * S2 - off, t * DS, n);
+            if (ACT) tma_load_4d(gs + Cfg::G_STAGE, &map_a, &full[st], x0 - off - HALO, y - tj * S2 - off, t * DS, n);
+        }
     };
     if (tid == 0)
         for (int t = 0; t < kNST && t < DS; ++t) issue(t);
@@ -264,29 +291,14 @@ corr_bwd_tiled_kernel(const __grid_constant__ CUtensorMap map_other,
         float g[DS][kPX];
 #pragma unroll
         for (int ti = 0; ti < DS; ++ti) {
-            if (WHICH == 1) {
-                float4 v0 = *reinterpret_cast<const float4 *>(gs + ti * GW);
-                float4 v1 = *reinterpret_cast<const float4 *>(gs + ti * GW + 4);
-                g[ti][0] = v0.x; g[ti][1] = v0.y; g[ti][2] = v0.z; g[ti][3] = v0.w;
-                g[ti][4] = v1.x; g[ti][5] = v1.y; g[ti][6] = v1.z; g[ti][7] = v1.w;
-            } else {
-                // gO[(tj,ti)][..][x' - (ti-DR)*S2 - off]; staged row starts at x0 - off - HALO
-                const float *q = gs + ti * GW + (2 * DR - ti) * S2;
-                if ((((2 * DR - ti) * S2) & 3) == 0) {
-                    float4 v0 = *reinterpret_cast<const float4 *>(q);
-                    float4 v1 = *reinterpret_cast<const float4 *>(q + 4);
-                    g[ti][0] = v0.x; g[ti][1] = v0.y; g[ti][2] = v0.z; g[ti][3] = v0.w;
-                    g[ti][4] = v1.x; g[ti][5] = v1.y; g[ti][6] = v1.z; g[ti][7] = v1.w;
-                } else if ((((2 * DR - ti) * S2) & 1) == 0) {
+            // WHICH == 2: gO[(tj,ti)][..][x' - (ti-DR)*S2 - off]; staged row starts at x0 - off - HALO
+            const int sh = (WHICH == 1) ? 0 : (2 * DR - ti) * S2;
+            lds_row8(gs + ti * GW + sh, sh, g[ti]);
+            if (ACT) {
+                float a[kPX];
+                lds_row8(gs + Cfg::G_STAGE + ti * GW + sh, sh, a);
 #pragma unroll
-                    for (int h = 0; h < 4; ++h) {
-                        float2 v = *reinterpret_cast<const float2 *>(q + 2 * h);
-                        g[ti][2 * h] = v.x; g[ti][2 * h + 1] = v.y;
-                    }
-                } else {
-#pragma unroll
-                    for (int i = 0; i < kPX; ++i) g[ti][i] = q[i];
-                }
+                for (int i = 0; i < kPX; ++i) g[ti][i] = a[i] > 0.f ? g[ti][i] : g[ti][i] * p.leaky;
             }
         }
 #pragma unroll
@@ -353,10 +365,11 @@ bool corr_tiled_supported(const CorrParams &p) {
     return false;
 }
 
+// bstride: elements between samples (0 = C*H*W, dense; larger = a channel range of a wider tensor)
 static int make_nchw_map(CUtensorMap *m, const float *base, int B, int C, int H, int W, int bw,
-                         int bc) {
+                         int bc, long bstride = 0) {
     uint64_t dims[4] = {(uint64_t)W, (uint64_t)H, (uint64_t)C, (uint64_t)B};
-    uint64_t strides[3] = {(uint64_t)W * 4, (uint64_t)W * H * 4, (uint64_t)W * H * C * 4};
+    uint64_t strides[3] = {(uint64_t)W * 4, (uint64_t)W * H * 4, (uint64_t)(bstride ? bstride : (long)W * H * C) * 4};
     uint32_t box[4] = {(uint32_t)bw, 1u, (uint32_t)bc, 1u};
     return make_tensor_map_f32(m, base, 4, dims, strides, box);
 }
@@ -381,24 +394,37 @@ static int launch_fwd(const float *in1, const float *in2, float *out, const Corr
     return check_launch("correlation_forward(tiled)");
 }
 
-template <int S2, int DR, int WHICH>
+template <int S2, int DR, int WHICH, bool ACT>
 static int launch_bwd(const float *other, const float *gout, float *gin, const CorrParams &p,
                       cudaStream_t st) {
-    using Cfg = BwdCfg<S2, DR, WHICH>;
-    CUtensorMap mo, mg;
+    using Cfg = BwdCfg<S2, DR, WHICH, ACT>;
+    static_assert(Cfg::SMEM <= 232448, "tiled backward stage ring exceeds the 227 KB of shared memory per block");
+    // gradOutput (and activation) maps: D planes per sample, p.g_bstride elements apart
+    CUtensorMap mo, mg, ma;
     int rc = make_nchw_map(&mo, other, p.B, p.C, p.H, p.W, Cfg::FW, Cfg::CB);
     if (rc) return rc;
-    rc = make_nchw_map(&mg, gout, p.B, p.D, p.oH, p.oW, Cfg::GW, Cfg::DS);
+    rc = make_nchw_map(&mg, gout, p.B, p.D, p.oH, p.oW, Cfg::GW, Cfg::DS, p.g_bstride);
     if (rc) return rc;
-    auto kern = corr_bwd_tiled_kernel<S2, DR, WHICH>;
+    if (ACT && (rc = make_nchw_map(&ma, p.act, p.B, p.D, p.oH, p.oW, Cfg::GW, Cfg::DS, p.g_bstride))) return rc;
+    if (!ACT) ma = mg;                           // not read
+    auto kern = corr_bwd_tiled_kernel<S2, DR, WHICH, ACT>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM);
     if (e != cudaSuccess) return fail((int)e, "correlation_backward: smem attribute (%s)", cudaGetErrorString(e));
     const int nxt = (p.W + kTW - 1) / kTW;
     const int ncb = (p.C + Cfg::CB - 1) / Cfg::CB;
     dim3 grid(nxt * ncb, p.H, p.B);
-    kern<<<grid, 256, Cfg::SMEM, st>>>(mo, mg, gin, p);
+    kern<<<grid, 256, Cfg::SMEM, st>>>(mo, mg, ma, gin, p);
     count_launch();
     return check_launch("correlation_backward(tiled)");
+}
+
+template <int S2, int DR, bool ACT>
+static int launch_bwd_both(const float *in1, const float *in2, const float *gout, float *gin1, float *gin2,
+                           const CorrParams &p, cudaStream_t st) {
+    int rc = 0;
+    if (gin1) rc = launch_bwd<S2, DR, 1, ACT>(in2, gout, gin1, p, st);
+    if (!rc && gin2) rc = launch_bwd<S2, DR, 2, ACT>(in1, gout, gin2, p, st);
+    return rc;
 }
 
 int corr_forward_tiled(const float *in1, const float *in2, float *out, const CorrParams &p,
@@ -416,15 +442,12 @@ int corr_forward_tiled(const float *in1, const float *in2, float *out, const Cor
 int corr_backward_tiled(const float *in1, const float *in2, const float *gout, float *gin1,
                         float *gin2, const CorrParams &p, cudaStream_t st) {
     if (!aligned16(in1) || !aligned16(in2) || !aligned16(gout) || (gin1 && !aligned16(gin1)) ||
-        (gin2 && !aligned16(gin2)))
+        (gin2 && !aligned16(gin2)) || (p.act && !aligned16(p.act)))
         return corr_backward_generic(in1, in2, gout, gin1, gin2, p, st);
-#define X(S2_, DR_)                                                                      \
-    if (p.s2 == S2_ && p.dr == DR_) {                                                    \
-        int rc = 0;                                                                      \
-        if (gin1) rc = launch_bwd<S2_, DR_, 1>(in2, gout, gin1, p, st);                  \
-        if (!rc && gin2) rc = launch_bwd<S2_, DR_, 2>(in1, gout, gin2, p, st);           \
-        return rc;                                                                       \
-    }
+#define X(S2_, DR_)                                                                                                     \
+    if (p.s2 == S2_ && p.dr == DR_)                                                                                     \
+        return p.act ? launch_bwd_both<S2_, DR_, true>(in1, in2, gout, gin1, gin2, p, st)                               \
+                     : launch_bwd_both<S2_, DR_, false>(in1, in2, gout, gin1, gin2, p, st);
     FN2_TILED_CONFIGS(X)
 #undef X
     return corr_backward_generic(in1, in2, gout, gin1, gin2, p, st);

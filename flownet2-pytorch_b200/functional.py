@@ -104,10 +104,11 @@ def correlation_forward(input1, input2, pad_size, kernel_size, max_displacement,
 
 
 def correlation_forward_cat(input1, input2, cat, ch_offset, leaky_slope, pad_size, kernel_size, max_displacement, stride1,
-                            stride2, corr_multiply=1):
+                            stride2, corr_multiply=1, return_workspace=False):
     """LeakyReLU(leaky_slope)(Correlation(...)(input1, input2)) written into cat[:, ch_offset : ch_offset + D] in place
     (FlowNetC.py:86-92: `torch.cat((out_conv_redir, corr_activation(corr)), 1)` without the activation pass and without
-    the copy).  cat: contiguous fp32 [B, channels, oH, oW]; its other channels are left alone.  Returns cat."""
+    the copy).  cat: contiguous fp32 [B, channels, oH, oW]; its other channels are left alone.  Returns cat, or
+    (cat, CorrWorkspace or None) with return_workspace=True, for correlation_backward_cat."""
     _require_cuda(input1, input2, cat)
     if input1.dim() != 4 or input1.shape != input2.shape:
         raise ValueError("correlation: input1/input2 must be 4-D with equal shapes")
@@ -125,7 +126,50 @@ def correlation_forward_cat(input1, input2, cat, ch_offset, leaky_slope, pad_siz
                                                   B, C, H, W, pad_size, kernel_size, max_displacement, stride1, stride2,
                                                   int(corr_multiply), _ptr(ws), ws_bytes, _stream(a)),
               "correlation_forward_cat")
-    return cat
+    if not return_workspace:
+        return cat
+    prm = (pad_size, kernel_size, max_displacement, stride1, stride2)
+    return cat, (CorrWorkspace(ws, _ws_key(a, b, prm)) if ws is not None else None)
+
+
+def _backward_workspace(a, b, prm, workspace):
+    """(buffer, bytes, has_split) for a tensor-core backward; the forward's workspace is reused when its key still
+    matches the inputs (same tensors, not modified in place since).  bytes == 0: the FMA kernels run."""
+    B, C, H, W = a.shape
+    ws_bytes = int(LIB.fn2b200_correlation_backward_workspace(B, C, H, W, *prm))
+    if not ws_bytes:
+        return None, 0, 0
+    have = int(workspace is not None and workspace.buf.numel() >= ws_bytes and workspace.buf.device == a.device
+               and workspace.key == _ws_key(a, b, prm))
+    return (workspace.buf if have else torch.empty(ws_bytes, dtype=torch.uint8, device=a.device)), ws_bytes, have
+
+
+def correlation_backward_cat(input1, input2, grad_cat, cat, ch_offset, leaky_slope, pad_size, kernel_size,
+                             max_displacement, stride1, stride2, corr_multiply=1, need1=True, need2=True, workspace=None):
+    """Backward of correlation_forward_cat: the input gradients of
+    cat[:, ch_offset : ch_offset + D] = LeakyReLU(leaky_slope)(Correlation(...)(input1, input2)), read straight from
+    grad_cat (the gradient of the whole concat) with LeakyReLU's derivative taken from `cat`, the buffer the forward
+    wrote (may be None when leaky_slope == 1).  One kernel launch on the tensor-core path when `workspace` is what
+    correlation_forward_cat(..., return_workspace=True) returned for the same inputs.  Returns (grad1, grad2)."""
+    _require_cuda(input1, input2, grad_cat, cat)
+    a, b, g = _f32c(input1), _f32c(input2), _f32c(grad_cat)
+    B, C, H, W = a.shape
+    D, oH, oW = correlation_out_shape(C, H, W, pad_size, kernel_size, max_displacement, stride1, stride2)
+    if g.dim() != 4 or (g.size(0), g.size(2), g.size(3)) != (B, oH, oW):
+        raise ValueError("correlation_backward_cat: grad_cat shape %s does not match [%d, channels, %d, %d]"
+                         % (tuple(g.shape), B, oH, oW))
+    if cat is not None:
+        _check_out(cat, g.shape, a.device, "correlation_backward_cat (cat)")
+    prm = (pad_size, kernel_size, max_displacement, stride1, stride2)
+    with torch.cuda.device_of(a):
+        g1 = torch.empty_like(a) if need1 else None
+        g2 = torch.empty_like(b) if need2 else None
+        ws, ws_bytes, have = _backward_workspace(a, b, prm, workspace)
+        check(LIB.fn2b200_correlation_backward_cat(_ptr(a), _ptr(b), _ptr(g), _ptr(cat), g.size(1), int(ch_offset),
+                                                   float(leaky_slope), _ptr(g1), _ptr(g2), B, C, H, W, *prm,
+                                                   int(corr_multiply), _ptr(ws), ws_bytes, have, _stream(a)),
+              "correlation_backward_cat")
+    return g1, g2
 
 
 def correlation_backward(input1, input2, grad_output, pad_size, kernel_size, max_displacement, stride1,
@@ -143,12 +187,9 @@ def correlation_backward(input1, input2, grad_output, pad_size, kernel_size, max
                 _check_out(o_, a.shape, a.device, "correlation_backward")
         g1 = (out1 if out1 is not None else torch.empty_like(a)) if need1 else None
         g2 = (out2 if out2 is not None else torch.empty_like(b)) if need2 else None
-        ws_bytes = int(LIB.fn2b200_correlation_backward_workspace(B, C, H, W, pad_size, kernel_size,
-                                                                  max_displacement, stride1, stride2))
+        ws, ws_bytes, have = _backward_workspace(a, b, (pad_size, kernel_size, max_displacement, stride1, stride2),
+                                                 workspace)
         if ws_bytes:
-            have = int(workspace is not None and workspace.buf.numel() >= ws_bytes and workspace.buf.device == a.device
-                       and workspace.key == _ws_key(a, b, (pad_size, kernel_size, max_displacement, stride1, stride2)))
-            ws = workspace.buf if have else torch.empty(ws_bytes, dtype=torch.uint8, device=a.device)
             check(LIB.fn2b200_correlation_backward_ws(_ptr(a), _ptr(b), _ptr(g), _ptr(g1), _ptr(g2), B, C, H, W,
                                                       pad_size, kernel_size, max_displacement, stride1, stride2,
                                                       int(corr_multiply), _ptr(ws), ws_bytes, have, _stream(a)),

@@ -94,6 +94,7 @@ int fn2b200_correlation_forward_ws(const float *input1, const float *input2, flo
  * first, then the 441 displacement channels), so that neither the activation's read-modify-write nor torch.cat's copy
  * of the cost volume happens.  leaky_slope = 1 writes the plain correlation.  workspace as in
  * fn2b200_correlation_forward_ws (NULL -> FP32-FMA kernels).  The other channels of `cat` are not touched.
+ * Its backward is fn2b200_correlation_backward_cat.
  */
 int fn2b200_correlation_forward_cat(const float *input1, const float *input2, float *cat, int cat_channels,
                                     int ch_offset, float leaky_slope, int B, int C, int H, int W, int pad_size,
@@ -112,6 +113,26 @@ int fn2b200_correlation_backward_ws(const float *input1, const float *input2, co
                                     int pad_size, int kernel_size, int max_displacement, int stride1,
                                     int stride2, int corr_type_multiply, void *workspace,
                                     size_t workspace_bytes, int workspace_has_split, void *stream);
+
+/*
+ * Backward of fn2b200_correlation_forward_cat: the input gradients of
+ *     cat[:, ch_offset : ch_offset + D] = LeakyReLU(leaky_slope)(correlation(input1, input2))
+ * given grad_cat, the gradient of the whole [B, cat_channels, oH, oW] concat buffer, and `cat`, the buffer the forward
+ * wrote (same layout; only its [ch_offset, ch_offset + D) channels are read).  Every gradOutput value is
+ *     gO[n,d,p] = grad_cat[n, ch_offset+d, p] * (cat[n, ch_offset+d, p] > 0 ? 1 : leaky_slope)
+ * (LeakyReLU's derivative read from its output, as torch's in-place LeakyReLU does), applied per element before any
+ * other arithmetic, so the result is bit-identical to fn2b200_correlation_backward_ws on that masked, dense gO.  The
+ * slice is read in place: no masked copy of the cost volume is written, and the tensor-core path stays one launch.
+ * leaky_slope = 1: no activation (cat may be NULL); leaky_slope < 0 -> FN2B200_EINVAL (the output's sign no longer gives
+ * the mask).  Workspace as in fn2b200_correlation_backward_ws (NULL -> FP32-FMA kernels; FN2B200_CORR_BWD=fma honoured).
+ * Channel range outside the buffer or a buffer of 2^31 elements or more -> FN2B200_EINVAL; stride1 != 1 ->
+ * FN2B200_EUNSUPPORTED; B == 0 is a no-op.
+ */
+int fn2b200_correlation_backward_cat(const float *input1, const float *input2, const float *grad_cat, const float *cat,
+                                     int cat_channels, int ch_offset, float leaky_slope, float *grad_input1,
+                                     float *grad_input2, int B, int C, int H, int W, int pad_size, int kernel_size,
+                                     int max_displacement, int stride1, int stride2, int corr_type_multiply,
+                                     void *workspace, size_t workspace_bytes, int workspace_has_split, void *stream);
 
 /*
  * grad_output: [B,D,oH,oW]; grad_input1, grad_input2: [B,C,H,W] (either may be NULL to skip it).
