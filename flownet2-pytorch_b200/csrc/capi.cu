@@ -7,15 +7,9 @@
 
 namespace fn2 {
 
-static int fill_corr_params(CorrParams &p, int B, int C, int H, int W, int pad, int k, int md,
-                            int s1, int s2) {
-    if (B < 0 || C <= 0 || H <= 0 || W <= 0)
-        return fail(FN2B200_EINVAL, "correlation: bad input shape [%d,%d,%d,%d]", B, C, H, W);
-    if (pad < 0 || k < 1 || md < 0 || s1 < 1 || s2 < 1)
-        return fail(FN2B200_EINVAL,
-                    "correlation: bad parameters pad=%d kernel_size=%d max_displacement=%d "
-                    "stride1=%d stride2=%d", pad, k, md, s1, s2);
-    p.B = B; p.C = C; p.H = H; p.W = W;
+// kr, dr, ds, D, oH, oW of a correlation with parameters already checked (s1, s2 >= 1).
+static void corr_geometry(CorrParams &p, int C, int H, int W, int pad, int k, int md, int s1, int s2) {
+    p.C = C; p.H = H; p.W = W;
     p.pad = pad; p.k = k; p.md = md; p.s1 = s1; p.s2 = s2;
     p.kr = (k - 1) / 2;
     p.dr = md / s2;
@@ -25,24 +19,115 @@ static int fill_corr_params(CorrParams &p, int B, int C, int H, int W, int pad, 
     // correlation_cuda.cc:33-34 -- float ceil of a float division
     p.oH = (int)ceilf((float)(H + 2 * pad - 2 * br) / (float)s1);
     p.oW = (int)ceilf((float)(W + 2 * pad - 2 * br) / (float)s1);
+}
+
+static int fill_corr_params(CorrParams &p, int B, int C, int H, int W, int pad, int k, int md,
+                            int s1, int s2) {
+    if (B < 0 || C <= 0 || H <= 0 || W <= 0)
+        return fail(FN2B200_EINVAL, "correlation: bad input shape [%d,%d,%d,%d]", B, C, H, W);
+    if (pad < 0 || k < 1 || md < 0 || s1 < 1 || s2 < 1)
+        return fail(FN2B200_EINVAL,
+                    "correlation: bad parameters pad=%d kernel_size=%d max_displacement=%d "
+                    "stride1=%d stride2=%d", pad, k, md, s1, s2);
+    p = CorrParams{};
+    p.B = B;
+    corr_geometry(p, C, H, W, pad, k, md, s1, s2);
     if (p.oH <= 0 || p.oW <= 0)
         return fail(FN2B200_EINVAL, "correlation: empty output (%d x %d); pad_size too small for "
                     "max_displacement/kernel_size", p.oH, p.oW);
     if ((int64_t)B * C * H * W >= (1LL << 31) || (int64_t)B * p.D * p.oH * p.oW >= (1LL << 31))
         return fail(FN2B200_EINVAL, "correlation: tensor exceeds 2^31 elements");
-    p.out_bstride = (long)p.D * p.oH * p.oW;
-    p.leaky = 1.f;
-    p.g_bstride = p.out_bstride;
-    p.act = nullptr;
     return 0;
 }
 
-// FN2B200_CORR_FWD = "fma" forces the FP32-FMA kernels, "tc" (default) uses tensor cores when the
-// configuration supports them and a workspace is supplied.  Read per call: no cached state.
-static bool tc_enabled() {
-    const char *e = getenv("FN2B200_CORR_FWD");
+// Every entry point's D correlation planes are channels [ch_offset, ch_offset + D) of a [B, cat_channels, oH, oW] buffer
+// (forward output, backward gradOutput) under LeakyReLU(leaky); the plain and *_ws ones use cat_channels = D, 0, 1.
+static int place_corr(CorrParams &p, const char *who, int cat_channels, int ch_offset, float leaky) {
+    if (ch_offset < 0 || cat_channels < ch_offset + p.D)
+        return fail(FN2B200_EINVAL, "%s: channels [%d, %d) do not fit a %d-channel buffer", who, ch_offset,
+                    ch_offset + p.D, cat_channels);
+    if ((int64_t)p.B * cat_channels * p.oH * p.oW >= (1LL << 31))
+        return fail(FN2B200_EINVAL, "%s: tensor exceeds 2^31 elements", who);
+    p.out_bstride = p.g_bstride = (long)cat_channels * p.oH * p.oW;
+    p.leaky = leaky;
+    return 0;
+}
+
+// FN2B200_CORR_FWD / FN2B200_CORR_BWD = "fma" keeps that direction on the FP32-FMA kernels; "tc" (default) lets it use
+// tensor cores.  Read per call: no cached state.
+static bool tc_enabled(bool backward) {
+    const char *e = getenv(backward ? "FN2B200_CORR_BWD" : "FN2B200_CORR_FWD");
     return !(e && (e[0] == 'f' || e[0] == 'F'));
 }
+
+enum CorrFamily { CORR_GENERIC = 0, CORR_TILED = 1, CORR_TC = 2 };      // the codes of fn2b200_correlation_path
+
+// The one rule that picks a correlation kernel family.  Tensor cores: a supported configuration, the direction's
+// environment switch and a large-enough workspace.  TMA-tiled FP32 FMA: a supported configuration and 16-byte aligned
+// operands (tensor-map bases and vector stores).  Everything else runs on the generic kernels.
+static CorrFamily corr_family(const CorrParams &p, bool backward, bool workspace_ok, bool aligned) {
+    if (workspace_ok && tc_enabled(backward) && corr_tc_supported(p)) return CORR_TC;
+    if (aligned && corr_tiled_supported(p)) return CORR_TILED;
+    return CORR_GENERIC;
+}
+
+static bool aligned16(const void *q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
+
+// Every correlation forward; dense = the plain [B, D, oH, oW] output.  `who` (the public name) prefixes error messages.
+static int corr_forward(const char *who, const float *in1, const float *in2, float *cat, bool dense, int cat_channels,
+                        int ch_offset, float leaky, int B, int C, int H, int W, int pad, int k, int md, int s1, int s2,
+                        void *workspace, size_t workspace_bytes, void *stream) {
+    CorrParams p;
+    int rc = fill_corr_params(p, B, C, H, W, pad, k, md, s1, s2);
+    if (rc || (rc = place_corr(p, who, dense ? p.D : cat_channels, ch_offset, leaky))) return rc;
+    if (B == 0) return 0;
+    if (!in1 || !in2 || !cat) return fail(FN2B200_ENULL, "%s: null pointer", who);
+    float *out = cat + (long)ch_offset * p.oH * p.oW;
+    if ((rc = bind_device_of(in1))) return rc;
+    // the tiled epilogue's 16-byte stores also need the output's batch stride to be a multiple of 4 elements
+    const bool aligned = aligned16(in1) && aligned16(in2) && aligned16(out) && !(p.out_bstride & 3);
+    cudaStream_t st = (cudaStream_t)stream;
+    switch (corr_family(p, false, workspace && workspace_bytes >= corr_tc_workspace_bytes(p), aligned)) {
+    case CORR_TC: return corr_forward_tc(in1, in2, out, p, workspace, workspace_bytes, st);
+    case CORR_TILED: return corr_forward_tiled(in1, in2, out, p, st);
+    default: return corr_forward_generic(in1, in2, out, p, st);
+    }
+}
+
+// Every correlation backward, as corr_forward; cat (the forward's activated output) is read only when leaky != 1.
+static int corr_backward(const char *who, const float *in1, const float *in2, const float *grad_cat, const float *cat,
+                         bool dense, int cat_channels, int ch_offset, float leaky, float *gin1, float *gin2, int B, int C,
+                         int H, int W, int pad, int k, int md, int s1, int s2, void *workspace, size_t workspace_bytes,
+                         int workspace_has_split, void *stream) {
+    CorrParams p;
+    int rc = fill_corr_params(p, B, C, H, W, pad, k, md, s1, s2);
+    if (rc) return rc;
+    if (!(leaky >= 0.f))
+        return fail(FN2B200_EINVAL, "%s: leaky_slope %g < 0 (the sign of the activated output no longer tells which "
+                    "side of 0 the correlation was on)", who, (double)leaky);
+    if ((rc = place_corr(p, who, dense ? p.D : cat_channels, ch_offset, leaky))) return rc;
+    if (s1 != 1)
+        return fail(FN2B200_EUNSUPPORTED, "%s: stride1=%d unsupported (the reference kernels index out of bounds for "
+                    "stride1 != 1, correlation_cuda_kernel.cu:163-164 vs :520)", who, s1);
+    if (B == 0) return 0;
+    const bool act = leaky != 1.f;
+    if (!in1 || !in2 || !grad_cat || (act && !cat)) return fail(FN2B200_ENULL, "%s: null pointer", who);
+    if (!gin1 && !gin2) return 0;
+    const long offset = (long)ch_offset * p.oH * p.oW;
+    const float *gout = grad_cat + offset;
+    p.act = act ? cat + offset : nullptr;
+    if ((rc = bind_device_of(in1))) return rc;
+    const bool aligned = aligned16(in1) && aligned16(in2) && aligned16(gout) && (!gin1 || aligned16(gin1)) &&
+                         (!gin2 || aligned16(gin2)) && (!p.act || aligned16(p.act));
+    cudaStream_t st = (cudaStream_t)stream;
+    switch (corr_family(p, true, workspace && workspace_bytes >= corr_tc_workspace_bytes(p), aligned)) {
+    case CORR_TC:
+        return corr_backward_tc(in1, in2, gout, gin1, gin2, p, workspace, workspace_bytes, workspace_has_split, st);
+    case CORR_TILED: return corr_backward_tiled(in1, in2, gout, gin1, gin2, p, st);
+    default: return corr_backward_generic(in1, in2, gout, gin1, gin2, p, st);
+    }
+}
+
 // FN2B200_RESAMPLE selects the Resample2d kernel family: "tile" (default; 2-D tiles, L1-cached gathers) or "row"
 // (round 1: one CTA = 256 pixels of a row; kept as the comparison point).
 enum { RS_TILE = 0, RS_ROW = 2 };
@@ -59,10 +144,6 @@ static int rs_scatter() {
     if (e && (e[0] == 'p' || e[0] == 'P')) return 1;
     return 2;
 }
-static bool tc_bwd_enabled() {
-    const char *e = getenv("FN2B200_CORR_BWD");
-    return !(e && (e[0] == 'f' || e[0] == 'F'));
-}
 
 }  // namespace fn2
 
@@ -77,114 +158,67 @@ uint64_t fn2b200_launch_count(void) { return launches_so_far(); }
 
 int fn2b200_correlation_out_shape(int C, int H, int W, int pad, int k, int md, int s1, int s2,
                                   int *D, int *oH, int *oW) {
-    CorrParams p;
-    // shape query must work for empty outputs too -> replicate arithmetic without the checks
+    // unlike fill_corr_params: any B, and empty outputs are reported rather than refused
     if (C <= 0 || H <= 0 || W <= 0 || pad < 0 || k < 1 || md < 0 || s1 < 1 || s2 < 1)
         return fail(FN2B200_EINVAL, "correlation_out_shape: bad parameters");
-    int kr = (k - 1) / 2, br = kr + md, dr = md / s2;
-    if (D) *D = (2 * dr + 1) * (2 * dr + 1);
-    if (oH) *oH = (int)ceilf((float)(H + 2 * pad - 2 * br) / (float)s1);
-    if (oW) *oW = (int)ceilf((float)(W + 2 * pad - 2 * br) / (float)s1);
-    (void)p;
+    CorrParams p;
+    corr_geometry(p, C, H, W, pad, k, md, s1, s2);
+    if (D) *D = p.D;
+    if (oH) *oH = p.oH;
+    if (oW) *oW = p.oW;
     return 0;
 }
 
 int fn2b200_correlation_path(int C, int H, int W, int pad, int k, int md, int s1, int s2) {
     CorrParams p;
     if (fill_corr_params(p, 1, C, H, W, pad, k, md, s1, s2)) return -1;
-    if (tc_enabled() && corr_tc_supported(p)) return 2;
-    return corr_tiled_supported(p) ? 1 : 0;
+    return corr_family(p, false, true, true);
 }
 
 int fn2b200_correlation_forward(const float *in1, const float *in2, float *out, int B, int C,
                                 int H, int W, int pad, int k, int md, int s1, int s2,
                                 int corr_type_multiply, void *stream) {
-    (void)corr_type_multiply;  // accepted and ignored: correlation_cuda_kernel.cu:369
-    CorrParams p;
-    int rc = fill_corr_params(p, B, C, H, W, pad, k, md, s1, s2);
-    if (rc) return rc;
-    if (B == 0) return 0;
-    if (!in1 || !in2 || !out) return fail(FN2B200_ENULL, "correlation_forward: null pointer");
-    if ((rc = bind_device_of(in1))) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (corr_tiled_supported(p)) return corr_forward_tiled(in1, in2, out, p, st);
-    return corr_forward_generic(in1, in2, out, p, st);
+    return fn2b200_correlation_forward_ws(in1, in2, out, B, C, H, W, pad, k, md, s1, s2, corr_type_multiply, nullptr, 0,
+                                          stream);
 }
 
 size_t fn2b200_correlation_forward_workspace(int B, int C, int H, int W, int pad, int k, int md, int s1,
                                              int s2) {
     CorrParams p;
     if (fill_corr_params(p, B, C, H, W, pad, k, md, s1, s2)) return 0;
-    if (!tc_enabled()) return 0;
+    if (!tc_enabled(false)) return 0;
     return corr_tc_workspace_bytes(p);
 }
 
 int fn2b200_correlation_forward_ws(const float *in1, const float *in2, float *out, int B, int C, int H,
                                    int W, int pad, int k, int md, int s1, int s2, int corr_type_multiply,
                                    void *workspace, size_t workspace_bytes, void *stream) {
-    CorrParams p;
-    int rc = fill_corr_params(p, B, C, H, W, pad, k, md, s1, s2);
-    if (rc) return rc;
-    if (B == 0) return 0;
-    if (!in1 || !in2 || !out) return fail(FN2B200_ENULL, "correlation_forward: null pointer");
-    if (workspace && tc_enabled() && corr_tc_supported(p) && workspace_bytes >= corr_tc_workspace_bytes(p)) {
-        if ((rc = bind_device_of(in1))) return rc;
-        return corr_forward_tc(in1, in2, out, p, workspace, workspace_bytes, (cudaStream_t)stream);
-    }
-    return fn2b200_correlation_forward(in1, in2, out, B, C, H, W, pad, k, md, s1, s2, corr_type_multiply, stream);
+    (void)corr_type_multiply;  // accepted and ignored: correlation_cuda_kernel.cu:369
+    return corr_forward("correlation_forward", in1, in2, out, true, 0, 0, 1.f, B, C, H, W, pad, k, md, s1, s2, workspace,
+                        workspace_bytes, stream);
 }
 
 int fn2b200_correlation_forward_cat(const float *in1, const float *in2, float *cat, int cat_channels, int ch_offset,
                                     float leaky_slope, int B, int C, int H, int W, int pad, int k, int md, int s1, int s2,
                                     int corr_type_multiply, void *workspace, size_t workspace_bytes, void *stream) {
     (void)corr_type_multiply;
-    CorrParams p;
-    int rc = fill_corr_params(p, B, C, H, W, pad, k, md, s1, s2);
-    if (rc) return rc;
-    if (ch_offset < 0 || cat_channels < ch_offset + p.D)
-        return fail(FN2B200_EINVAL, "correlation_forward_cat: channels [%d, %d) do not fit a %d-channel buffer", ch_offset,
-                    ch_offset + p.D, cat_channels);
-    if ((int64_t)B * cat_channels * p.oH * p.oW >= (1LL << 31))
-        return fail(FN2B200_EINVAL, "correlation_forward_cat: tensor exceeds 2^31 elements");
-    if (B == 0) return 0;
-    if (!in1 || !in2 || !cat) return fail(FN2B200_ENULL, "correlation_forward_cat: null pointer");
-    p.out_bstride = (long)cat_channels * p.oH * p.oW;
-    p.leaky = leaky_slope;
-    float *out = cat + (long)ch_offset * p.oH * p.oW;
-    if ((rc = bind_device_of(in1))) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (workspace && tc_enabled() && corr_tc_supported(p) && workspace_bytes >= corr_tc_workspace_bytes(p))
-        return corr_forward_tc(in1, in2, out, p, workspace, workspace_bytes, st);
-    if (corr_tiled_supported(p)) return corr_forward_tiled(in1, in2, out, p, st);
-    return corr_forward_generic(in1, in2, out, p, st);
+    return corr_forward("correlation_forward_cat", in1, in2, cat, false, cat_channels, ch_offset, leaky_slope, B, C, H, W,
+                        pad, k, md, s1, s2, workspace, workspace_bytes, stream);
 }
 
 int fn2b200_correlation_backward(const float *in1, const float *in2, const float *gout,
                                  float *gin1, float *gin2, int B, int C, int H, int W, int pad,
                                  int k, int md, int s1, int s2, int corr_type_multiply,
                                  void *stream) {
-    (void)corr_type_multiply;
-    CorrParams p;
-    int rc = fill_corr_params(p, B, C, H, W, pad, k, md, s1, s2);
-    if (rc) return rc;
-    if (s1 != 1)
-        return fail(FN2B200_EUNSUPPORTED,
-                    "correlation_backward: stride1=%d unsupported (the reference kernels index out "
-                    "of bounds for stride1 != 1, correlation_cuda_kernel.cu:163-164 vs :520)", s1);
-    if (B == 0) return 0;
-    if (!in1 || !in2 || !gout) return fail(FN2B200_ENULL, "correlation_backward: null pointer");
-    if (!gin1 && !gin2) return 0;
-    if ((rc = bind_device_of(in1))) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (corr_tiled_supported(p)) return corr_backward_tiled(in1, in2, gout, gin1, gin2, p, st);
-    return corr_backward_generic(in1, in2, gout, gin1, gin2, p, st);
+    return fn2b200_correlation_backward_ws(in1, in2, gout, gin1, gin2, B, C, H, W, pad, k, md, s1, s2, corr_type_multiply,
+                                           nullptr, 0, 0, stream);
 }
 
 size_t fn2b200_correlation_backward_workspace(int B, int C, int H, int W, int pad, int k, int md, int s1,
                                               int s2) {
     CorrParams p;
     if (fill_corr_params(p, B, C, H, W, pad, k, md, s1, s2)) return 0;
-    if (!tc_bwd_enabled()) return 0;
+    if (!tc_enabled(true)) return 0;
     return corr_tc_workspace_bytes(p);
 }
 
@@ -192,19 +226,9 @@ int fn2b200_correlation_backward_ws(const float *in1, const float *in2, const fl
                                     float *gin2, int B, int C, int H, int W, int pad, int k, int md, int s1,
                                     int s2, int corr_type_multiply, void *workspace, size_t workspace_bytes,
                                     int workspace_has_split, void *stream) {
-    CorrParams p;
-    int rc = fill_corr_params(p, B, C, H, W, pad, k, md, s1, s2);
-    if (rc) return rc;
-    if (workspace && tc_bwd_enabled() && corr_tc_supported(p) && workspace_bytes >= corr_tc_workspace_bytes(p)) {
-        if (B == 0) return 0;
-        if (!in1 || !in2 || !gout) return fail(FN2B200_ENULL, "correlation_backward: null pointer");
-        if (!gin1 && !gin2) return 0;
-        if ((rc = bind_device_of(in1))) return rc;
-        return corr_backward_tc(in1, in2, gout, gin1, gin2, p, workspace, workspace_bytes, workspace_has_split,
-                                (cudaStream_t)stream);
-    }
-    return fn2b200_correlation_backward(in1, in2, gout, gin1, gin2, B, C, H, W, pad, k, md, s1, s2,
-                                        corr_type_multiply, stream);
+    (void)corr_type_multiply;
+    return corr_backward("correlation_backward", in1, in2, gout, nullptr, true, 0, 0, 1.f, gin1, gin2, B, C, H, W, pad, k,
+                         md, s1, s2, workspace, workspace_bytes, workspace_has_split, stream);
 }
 
 int fn2b200_correlation_backward_cat(const float *in1, const float *in2, const float *grad_cat, const float *cat,
@@ -212,35 +236,9 @@ int fn2b200_correlation_backward_cat(const float *in1, const float *in2, const f
                                      int C, int H, int W, int pad, int k, int md, int s1, int s2, int corr_type_multiply,
                                      void *workspace, size_t workspace_bytes, int workspace_has_split, void *stream) {
     (void)corr_type_multiply;
-    CorrParams p;
-    int rc = fill_corr_params(p, B, C, H, W, pad, k, md, s1, s2);
-    if (rc) return rc;
-    if (!(leaky_slope >= 0.f))
-        return fail(FN2B200_EINVAL, "correlation_backward_cat: leaky_slope %g < 0 (the sign of the activated output no "
-                    "longer tells which side of 0 the correlation was on)", (double)leaky_slope);
-    if (ch_offset < 0 || cat_channels < ch_offset + p.D)
-        return fail(FN2B200_EINVAL, "correlation_backward_cat: channels [%d, %d) do not fit a %d-channel buffer", ch_offset,
-                    ch_offset + p.D, cat_channels);
-    if ((int64_t)B * cat_channels * p.oH * p.oW >= (1LL << 31))
-        return fail(FN2B200_EINVAL, "correlation_backward_cat: tensor exceeds 2^31 elements");
-    if (s1 != 1)
-        return fail(FN2B200_EUNSUPPORTED, "correlation_backward_cat: stride1=%d unsupported (as fn2b200_correlation_backward)",
-                    s1);
-    if (B == 0) return 0;
-    const bool act = leaky_slope != 1.f;
-    if (!in1 || !in2 || !grad_cat || (act && !cat)) return fail(FN2B200_ENULL, "correlation_backward_cat: null pointer");
-    if (!gin1 && !gin2) return 0;
-    const long plane = (long)p.oH * p.oW;
-    const float *gout = grad_cat + ch_offset * plane;
-    p.g_bstride = cat_channels * plane;
-    p.act = act ? cat + ch_offset * plane : nullptr;
-    p.leaky = leaky_slope;
-    if ((rc = bind_device_of(in1))) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    if (workspace && tc_bwd_enabled() && corr_tc_supported(p) && workspace_bytes >= corr_tc_workspace_bytes(p))
-        return corr_backward_tc(in1, in2, gout, gin1, gin2, p, workspace, workspace_bytes, workspace_has_split, st);
-    if (corr_tiled_supported(p)) return corr_backward_tiled(in1, in2, gout, gin1, gin2, p, st);
-    return corr_backward_generic(in1, in2, gout, gin1, gin2, p, st);
+    return corr_backward("correlation_backward_cat", in1, in2, grad_cat, cat, false, cat_channels, ch_offset, leaky_slope,
+                         gin1, gin2, B, C, H, W, pad, k, md, s1, s2, workspace, workspace_bytes, workspace_has_split,
+                         stream);
 }
 
 // shared argument checks of the fused warp-concat entry points

@@ -190,7 +190,8 @@ int corr_forward_generic(const float *in1, const float *in2, float *out, const C
                          cudaStream_t st);
 int corr_backward_generic(const float *in1, const float *in2, const float *gout, float *gin1,
                           float *gin2, const CorrParams &p, cudaStream_t st);
-// TMA-tiled FMA kernels: kernel_size == 1, stride1 == 1, (s2, dr) in the instantiated set, W % 4 == 0.
+// TMA-tiled FMA kernels: kernel_size == 1, stride1 == 1, (s2, dr) in the instantiated set, W % 4 == 0; the caller also
+// guarantees 16-byte aligned operands (capi.cu's corr_family chooses the family).
 bool corr_tiled_supported(const CorrParams &p);
 int corr_forward_tiled(const float *in1, const float *in2, float *out, const CorrParams &p,
                        cudaStream_t st);

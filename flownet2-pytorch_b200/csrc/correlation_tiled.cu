@@ -348,8 +348,6 @@ corr_bwd_tiled_kernel(const __grid_constant__ CUtensorMap map_other,
 // ------------------------------------------------------------------------------------------------
 // Host side
 // ------------------------------------------------------------------------------------------------
-static inline bool aligned16(const void *q) { return (reinterpret_cast<uintptr_t>(q) & 15) == 0; }
-
 // (stride2, displacement radius) pairs with a compiled tiled kernel; the x halo dr*s2 must be a
 // multiple of 4 (TMA traps on a dim-0 start coordinate that is not 16-byte aligned -- measured).
 #define FN2_TILED_CONFIGS(X) X(2, 10) X(2, 4) X(1, 4) X(2, 2)
@@ -429,28 +427,21 @@ static int launch_bwd_both(const float *in1, const float *in2, const float *gout
 
 int corr_forward_tiled(const float *in1, const float *in2, float *out, const CorrParams &p,
                        cudaStream_t st) {
-    // the epilogue's st.global.v4 needs 16-byte aligned output rows: base, batch stride and plane size
-    if (!aligned16(out) || (p.out_bstride & 3)) return corr_forward_generic(in1, in2, out, p, st);
-    if (!aligned16(in1) || !aligned16(in2))
-        return corr_forward_generic(in1, in2, out, p, st);
 #define X(S2_, DR_) if (p.s2 == S2_ && p.dr == DR_) return launch_fwd<S2_, DR_>(in1, in2, out, p, st);
     FN2_TILED_CONFIGS(X)
 #undef X
-    return corr_forward_generic(in1, in2, out, p, st);
+    return fail(FN2B200_EUNSUPPORTED, "correlation_forward(tiled): no kernel for stride2=%d, dr=%d", p.s2, p.dr);
 }
 
 int corr_backward_tiled(const float *in1, const float *in2, const float *gout, float *gin1,
                         float *gin2, const CorrParams &p, cudaStream_t st) {
-    if (!aligned16(in1) || !aligned16(in2) || !aligned16(gout) || (gin1 && !aligned16(gin1)) ||
-        (gin2 && !aligned16(gin2)) || (p.act && !aligned16(p.act)))
-        return corr_backward_generic(in1, in2, gout, gin1, gin2, p, st);
 #define X(S2_, DR_)                                                                                                     \
     if (p.s2 == S2_ && p.dr == DR_)                                                                                     \
         return p.act ? launch_bwd_both<S2_, DR_, true>(in1, in2, gout, gin1, gin2, p, st)                               \
                      : launch_bwd_both<S2_, DR_, false>(in1, in2, gout, gin1, gin2, p, st);
     FN2_TILED_CONFIGS(X)
 #undef X
-    return corr_backward_generic(in1, in2, gout, gin1, gin2, p, st);
+    return fail(FN2B200_EUNSUPPORTED, "correlation_backward(tiled): no kernel for stride2=%d, dr=%d", p.s2, p.dr);
 }
 
 }  // namespace fn2

@@ -67,40 +67,60 @@ def _ws_key(a, b, prm):
     return (a.data_ptr(), b.data_ptr(), a._version, b._version, tuple(a.shape)) + tuple(prm)
 
 
-def correlation_forward(input1, input2, pad_size, kernel_size, max_displacement, stride1, stride2,
-                        corr_multiply=1, out=None, return_workspace=False):
-    _require_cuda(input1, input2)
+def _corr_inputs(input1, input2, prm, *others):
+    """(input1, input2) as contiguous fp32 and the correlation's (D, oH, oW); every tensor must be on CUDA."""
+    _require_cuda(input1, input2, *others)
     if input1.dim() != 4 or input1.shape != input2.shape:
         raise ValueError("correlation: input1/input2 must be 4-D with equal shapes, got %s and %s"
                          % (tuple(input1.shape), tuple(input2.shape)))
     a, b = _f32c(input1), _f32c(input2)
+    return a, b, correlation_out_shape(a.size(1), a.size(2), a.size(3), *prm)
+
+
+def _corr_forward(a, b, cat, ch_offset, leaky_slope, prm, corr_multiply, who):
+    """LeakyReLU(leaky_slope)(correlation) into cat[:, ch_offset : ch_offset + D] with one
+    fn2b200_correlation_forward_cat call.  Returns the tensor-core workspace as a CorrWorkspace, or None."""
     B, C, H, W = a.shape
-    D, oH, oW = correlation_out_shape(C, H, W, pad_size, kernel_size, max_displacement, stride1, stride2)
-    if oH <= 0 or oW <= 0:
-        raise ValueError("correlation: empty output (%d x %d) for input %dx%d, pad_size=%d, "
-                         "max_displacement=%d, kernel_size=%d" % (oH, oW, H, W, pad_size, max_displacement, kernel_size))
     with torch.cuda.device_of(a):
-        if out is None:
-            out = torch.empty((B, D, oH, oW), dtype=torch.float32, device=a.device)
-        else:
-            _check_out(out, (B, D, oH, oW), a.device, "correlation_forward")
-        ws_bytes = int(LIB.fn2b200_correlation_forward_workspace(B, C, H, W, pad_size, kernel_size, max_displacement,
-                                                                 stride1, stride2))
-        if ws_bytes:
-            # scratch for the tensor-core path's bf16 hi/lo operands (the analogue of the reference's
-            # rbot1/rbot2, correlation.py:20-21); the caching allocator keeps it stream-ordered
-            ws = torch.empty(ws_bytes, dtype=torch.uint8, device=a.device)
-            check(LIB.fn2b200_correlation_forward_ws(_ptr(a), _ptr(b), _ptr(out), B, C, H, W, pad_size, kernel_size,
-                                                     max_displacement, stride1, stride2, int(corr_multiply),
-                                                     _ptr(ws), ws_bytes, _stream(a)),
-                  "correlation_forward")
-            wsobj = CorrWorkspace(ws, _ws_key(a, b, (pad_size, kernel_size, max_displacement, stride1, stride2)))
-        else:
-            check(LIB.fn2b200_correlation_forward(_ptr(a), _ptr(b), _ptr(out), B, C, H, W, pad_size, kernel_size,
-                                                  max_displacement, stride1, stride2, int(corr_multiply), _stream(a)),
-                  "correlation_forward")
-            wsobj = None
-    return (out, wsobj) if return_workspace else out
+        ws_bytes = int(LIB.fn2b200_correlation_forward_workspace(B, C, H, W, *prm))
+        # scratch for the tensor-core path's bf16 hi/lo operands (the analogue of the reference's
+        # rbot1/rbot2, correlation.py:20-21); the caching allocator keeps it stream-ordered
+        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=a.device) if ws_bytes else None
+        check(LIB.fn2b200_correlation_forward_cat(_ptr(a), _ptr(b), _ptr(cat), cat.size(1), int(ch_offset), float(leaky_slope),
+                                                  B, C, H, W, *prm, int(corr_multiply), _ptr(ws), ws_bytes, _stream(a)), who)
+    return CorrWorkspace(ws, _ws_key(a, b, prm)) if ws is not None else None
+
+
+def _corr_backward(a, b, g, cat, ch_offset, leaky_slope, prm, corr_multiply, g1, g2, workspace, who):
+    """g1, g2 (either may be None) from one fn2b200_correlation_backward_cat call, the correlation's gradient being
+    g[:, ch_offset : ch_offset + D].  The forward's workspace is reused when its key still matches the inputs (same
+    tensors, not modified in place since): the tensor-core backward then skips the split pass."""
+    B, C, H, W = a.shape
+    with torch.cuda.device_of(a):
+        ws_bytes = int(LIB.fn2b200_correlation_backward_workspace(B, C, H, W, *prm))
+        have = int(bool(ws_bytes) and workspace is not None and workspace.buf.numel() >= ws_bytes
+                   and workspace.buf.device == a.device and workspace.key == _ws_key(a, b, prm))
+        ws = workspace.buf if have else (torch.empty(ws_bytes, dtype=torch.uint8, device=a.device) if ws_bytes else None)
+        check(LIB.fn2b200_correlation_backward_cat(_ptr(a), _ptr(b), _ptr(g), _ptr(cat), g.size(1), int(ch_offset),
+                                                   float(leaky_slope), _ptr(g1), _ptr(g2), B, C, H, W, *prm,
+                                                   int(corr_multiply), _ptr(ws), ws_bytes, have, _stream(a)), who)
+    return g1, g2
+
+
+def correlation_forward(input1, input2, pad_size, kernel_size, max_displacement, stride1, stride2,
+                        corr_multiply=1, out=None, return_workspace=False):
+    prm = (pad_size, kernel_size, max_displacement, stride1, stride2)
+    a, b, (D, oH, oW) = _corr_inputs(input1, input2, prm)
+    if oH <= 0 or oW <= 0:
+        raise ValueError("correlation: empty output (%d x %d) for input %dx%d, pad_size=%d, max_displacement=%d, "
+                         "kernel_size=%d" % (oH, oW, a.size(2), a.size(3), pad_size, max_displacement, kernel_size))
+    shape = (a.size(0), D, oH, oW)
+    if out is None:
+        out = torch.empty(shape, dtype=torch.float32, device=a.device)
+    else:
+        _check_out(out, shape, a.device, "correlation_forward")
+    ws = _corr_forward(a, b, out, 0, 1.0, prm, corr_multiply, "correlation_forward")
+    return (out, ws) if return_workspace else out
 
 
 def correlation_forward_cat(input1, input2, cat, ch_offset, leaky_slope, pad_size, kernel_size, max_displacement, stride1,
@@ -109,39 +129,13 @@ def correlation_forward_cat(input1, input2, cat, ch_offset, leaky_slope, pad_siz
     (FlowNetC.py:86-92: `torch.cat((out_conv_redir, corr_activation(corr)), 1)` without the activation pass and without
     the copy).  cat: contiguous fp32 [B, channels, oH, oW]; its other channels are left alone.  Returns cat, or
     (cat, CorrWorkspace or None) with return_workspace=True, for correlation_backward_cat."""
-    _require_cuda(input1, input2, cat)
-    if input1.dim() != 4 or input1.shape != input2.shape:
-        raise ValueError("correlation: input1/input2 must be 4-D with equal shapes")
-    a, b = _f32c(input1), _f32c(input2)
-    B, C, H, W = a.shape
-    D, oH, oW = correlation_out_shape(C, H, W, pad_size, kernel_size, max_displacement, stride1, stride2)
+    prm = (pad_size, kernel_size, max_displacement, stride1, stride2)
+    a, b, (D, oH, oW) = _corr_inputs(input1, input2, prm, cat)
     if cat.dim() != 4:
         raise ValueError("correlation_forward_cat: cat must be 4-D")
-    _check_out(cat, (B, cat.size(1), oH, oW), a.device, "correlation_forward_cat")
-    with torch.cuda.device_of(a):
-        ws_bytes = int(LIB.fn2b200_correlation_forward_workspace(B, C, H, W, pad_size, kernel_size, max_displacement,
-                                                                 stride1, stride2))
-        ws = torch.empty(ws_bytes, dtype=torch.uint8, device=a.device) if ws_bytes else None
-        check(LIB.fn2b200_correlation_forward_cat(_ptr(a), _ptr(b), _ptr(cat), cat.size(1), int(ch_offset), float(leaky_slope),
-                                                  B, C, H, W, pad_size, kernel_size, max_displacement, stride1, stride2,
-                                                  int(corr_multiply), _ptr(ws), ws_bytes, _stream(a)),
-              "correlation_forward_cat")
-    if not return_workspace:
-        return cat
-    prm = (pad_size, kernel_size, max_displacement, stride1, stride2)
-    return cat, (CorrWorkspace(ws, _ws_key(a, b, prm)) if ws is not None else None)
-
-
-def _backward_workspace(a, b, prm, workspace):
-    """(buffer, bytes, has_split) for a tensor-core backward; the forward's workspace is reused when its key still
-    matches the inputs (same tensors, not modified in place since).  bytes == 0: the FMA kernels run."""
-    B, C, H, W = a.shape
-    ws_bytes = int(LIB.fn2b200_correlation_backward_workspace(B, C, H, W, *prm))
-    if not ws_bytes:
-        return None, 0, 0
-    have = int(workspace is not None and workspace.buf.numel() >= ws_bytes and workspace.buf.device == a.device
-               and workspace.key == _ws_key(a, b, prm))
-    return (workspace.buf if have else torch.empty(ws_bytes, dtype=torch.uint8, device=a.device)), ws_bytes, have
+    _check_out(cat, (a.size(0), cat.size(1), oH, oW), a.device, "correlation_forward_cat")
+    ws = _corr_forward(a, b, cat, ch_offset, leaky_slope, prm, corr_multiply, "correlation_forward_cat")
+    return (cat, ws) if return_workspace else cat
 
 
 def correlation_backward_cat(input1, input2, grad_cat, cat, ch_offset, leaky_slope, pad_size, kernel_size,
@@ -151,55 +145,34 @@ def correlation_backward_cat(input1, input2, grad_cat, cat, ch_offset, leaky_slo
     grad_cat (the gradient of the whole concat) with LeakyReLU's derivative taken from `cat`, the buffer the forward
     wrote (may be None when leaky_slope == 1).  One kernel launch on the tensor-core path when `workspace` is what
     correlation_forward_cat(..., return_workspace=True) returned for the same inputs.  Returns (grad1, grad2)."""
-    _require_cuda(input1, input2, grad_cat, cat)
-    a, b, g = _f32c(input1), _f32c(input2), _f32c(grad_cat)
-    B, C, H, W = a.shape
-    D, oH, oW = correlation_out_shape(C, H, W, pad_size, kernel_size, max_displacement, stride1, stride2)
-    if g.dim() != 4 or (g.size(0), g.size(2), g.size(3)) != (B, oH, oW):
+    prm = (pad_size, kernel_size, max_displacement, stride1, stride2)
+    a, b, (D, oH, oW) = _corr_inputs(input1, input2, prm, grad_cat, cat)
+    g = _f32c(grad_cat)
+    if g.dim() != 4 or (g.size(0), g.size(2), g.size(3)) != (a.size(0), oH, oW):
         raise ValueError("correlation_backward_cat: grad_cat shape %s does not match [%d, channels, %d, %d]"
-                         % (tuple(g.shape), B, oH, oW))
+                         % (tuple(g.shape), a.size(0), oH, oW))
     if cat is not None:
         _check_out(cat, g.shape, a.device, "correlation_backward_cat (cat)")
-    prm = (pad_size, kernel_size, max_displacement, stride1, stride2)
-    with torch.cuda.device_of(a):
-        g1 = torch.empty_like(a) if need1 else None
-        g2 = torch.empty_like(b) if need2 else None
-        ws, ws_bytes, have = _backward_workspace(a, b, prm, workspace)
-        check(LIB.fn2b200_correlation_backward_cat(_ptr(a), _ptr(b), _ptr(g), _ptr(cat), g.size(1), int(ch_offset),
-                                                   float(leaky_slope), _ptr(g1), _ptr(g2), B, C, H, W, *prm,
-                                                   int(corr_multiply), _ptr(ws), ws_bytes, have, _stream(a)),
-              "correlation_backward_cat")
-    return g1, g2
+    g1 = torch.empty_like(a) if need1 else None
+    g2 = torch.empty_like(b) if need2 else None
+    return _corr_backward(a, b, g, cat, ch_offset, leaky_slope, prm, corr_multiply, g1, g2, workspace,
+                          "correlation_backward_cat")
 
 
 def correlation_backward(input1, input2, grad_output, pad_size, kernel_size, max_displacement, stride1,
                          stride2, corr_multiply=1, need1=True, need2=True, out1=None, out2=None, workspace=None):
-    _require_cuda(input1, input2, grad_output)
-    a, b, g = _f32c(input1), _f32c(input2), _f32c(grad_output)
-    B, C, H, W = a.shape
-    D, oH, oW = correlation_out_shape(C, H, W, pad_size, kernel_size, max_displacement, stride1, stride2)
-    if tuple(g.shape) != (B, D, oH, oW):
+    prm = (pad_size, kernel_size, max_displacement, stride1, stride2)
+    a, b, (D, oH, oW) = _corr_inputs(input1, input2, prm, grad_output)
+    g = _f32c(grad_output)
+    if tuple(g.shape) != (a.size(0), D, oH, oW):
         raise ValueError("correlation_backward: grad_output shape %s != expected %s"
-                         % (tuple(g.shape), (B, D, oH, oW)))
-    with torch.cuda.device_of(a):
-        for o_ in (out1, out2):
-            if o_ is not None:
-                _check_out(o_, a.shape, a.device, "correlation_backward")
-        g1 = (out1 if out1 is not None else torch.empty_like(a)) if need1 else None
-        g2 = (out2 if out2 is not None else torch.empty_like(b)) if need2 else None
-        ws, ws_bytes, have = _backward_workspace(a, b, (pad_size, kernel_size, max_displacement, stride1, stride2),
-                                                 workspace)
-        if ws_bytes:
-            check(LIB.fn2b200_correlation_backward_ws(_ptr(a), _ptr(b), _ptr(g), _ptr(g1), _ptr(g2), B, C, H, W,
-                                                      pad_size, kernel_size, max_displacement, stride1, stride2,
-                                                      int(corr_multiply), _ptr(ws), ws_bytes, have, _stream(a)),
-                  "correlation_backward")
-        else:
-            check(LIB.fn2b200_correlation_backward(_ptr(a), _ptr(b), _ptr(g), _ptr(g1), _ptr(g2), B, C, H, W,
-                                                   pad_size, kernel_size, max_displacement, stride1, stride2,
-                                                   int(corr_multiply), _stream(a)),
-                  "correlation_backward")
-    return g1, g2
+                         % (tuple(g.shape), (a.size(0), D, oH, oW)))
+    for o_ in (out1, out2):
+        if o_ is not None:
+            _check_out(o_, a.shape, a.device, "correlation_backward")
+    g1 = (out1 if out1 is not None else torch.empty_like(a)) if need1 else None
+    g2 = (out2 if out2 is not None else torch.empty_like(b)) if need2 else None
+    return _corr_backward(a, b, g, None, 0, 1.0, prm, corr_multiply, g1, g2, workspace, "correlation_backward")
 
 
 def _img_strides(img):

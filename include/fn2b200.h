@@ -61,10 +61,9 @@ int fn2b200_correlation_out_shape(int C, int H, int W, int pad_size, int kernel_
                                   int *oH, int *oW);
 
 /*
- * input1, input2: [B,C,H,W]; output: [B,D,oH,oW].
- * corr_type_multiply is accepted and ignored, exactly as in the reference
- * (correlation_cuda_kernel.cu:369).  No padded/transposed scratch tensors are needed (the
- * reference's rInput1/rInput2 have no counterpart here).
+ * fn2b200_correlation_forward_cat with cat_channels = D, ch_offset = 0, leaky_slope = 1 and no workspace (FP32-FMA
+ * kernels): output [B,D,oH,oW].  No padded/transposed scratch tensors are needed (the reference's rInput1/rInput2 have
+ * no counterpart here).
  */
 int fn2b200_correlation_forward(const float *input1, const float *input2, float *output, int B,
                                 int C, int H, int W, int pad_size, int kernel_size,
@@ -72,14 +71,9 @@ int fn2b200_correlation_forward(const float *input1, const float *input2, float 
                                 int corr_type_multiply, void *stream);
 
 /*
- * Tensor-core forward (wgmma, bf16 hi/lo operand split, fp32 accumulation in registers; error ~1e-5
- * relative, inside the 1e-4 contract).  It needs scratch for the split operands:
- * fn2b200_correlation_forward_workspace() returns the bytes required (0 = this configuration runs
- * on the FP32-FMA kernels; set the environment variable FN2B200_CORR_FWD=fma to force that), and
- * fn2b200_correlation_forward_ws() is fn2b200_correlation_forward() plus a 128-byte-aligned device
- * workspace of at least that size (NULL / too small -> the FMA kernels).  The workspace plays the
- * role of the reference's rInput1/rInput2 scratch tensors (correlation_cuda.cc:36-41) and may be
- * reused or freed (stream-ordered) as soon as the call returns.
+ * fn2b200_correlation_forward_workspace() returns the workspace bytes of the tensor-core forward (0 = the FP32-FMA
+ * kernels run: configuration not supported, or FN2B200_CORR_FWD=fma).  fn2b200_correlation_forward_ws() equals
+ * fn2b200_correlation_forward_cat with cat_channels = D, ch_offset = 0, leaky_slope = 1: output [B,D,oH,oW].
  */
 size_t fn2b200_correlation_forward_workspace(int B, int C, int H, int W, int pad_size, int kernel_size,
                                              int max_displacement, int stride1, int stride2);
@@ -89,12 +83,21 @@ int fn2b200_correlation_forward_ws(const float *input1, const float *input2, flo
                                    size_t workspace_bytes, void *stream);
 
 /*
- * SURVEY 8(f)-2 (FlowNetC.py:86-92): the forward writing LeakyReLU(leaky_slope)(correlation) straight into channels
- * [ch_offset, ch_offset + D) of a [B, cat_channels, oH, oW] concat buffer (FlowNetC: 473 channels, conv_redir's 32
- * first, then the 441 displacement channels), so that neither the activation's read-modify-write nor torch.cat's copy
- * of the cost volume happens.  leaky_slope = 1 writes the plain correlation.  workspace as in
- * fn2b200_correlation_forward_ws (NULL -> FP32-FMA kernels).  The other channels of `cat` are not touched.
- * Its backward is fn2b200_correlation_backward_cat.
+ * The correlation forward.  input1, input2: [B,C,H,W]; cat: [B, cat_channels, oH, oW].  Writes
+ * LeakyReLU(leaky_slope)(correlation) into channels [ch_offset, ch_offset + D) of cat and leaves its other channels
+ * untouched; leaky_slope = 1 writes the plain correlation.  SURVEY 8(f)-2 (FlowNetC.py:86-92): FlowNetC's 473-channel
+ * concat holds conv_redir's 32 channels first, then the 441 displacement channels, so neither the activation's
+ * read-modify-write nor torch.cat's copy of the cost volume happens.
+ * Tensor cores (wgmma, bf16 hi/lo operand split, fp32 accumulation in registers; error ~1e-5 relative, inside the 1e-4
+ * contract) run when the configuration supports them and the workspace holds at least
+ * fn2b200_correlation_forward_workspace() bytes; it must then be 128-byte aligned (else FN2B200_EINVAL).  A NULL or
+ * smaller workspace, or FN2B200_CORR_FWD=fma, selects the FP32-FMA kernels.  The workspace plays the role of the
+ * reference's rInput1/rInput2 scratch tensors (correlation_cuda.cc:36-41) and may be reused or freed (stream-ordered)
+ * as soon as the call returns.  corr_type_multiply is accepted and ignored, exactly as in the reference
+ * (correlation_cuda_kernel.cu:369).
+ * Bad shape or parameters, an empty output, a channel range outside the buffer or a tensor of 2^31 elements or more ->
+ * FN2B200_EINVAL; NULL input1, input2 or cat -> FN2B200_ENULL; B == 0 is a no-op.  Its backward is
+ * fn2b200_correlation_backward_cat.
  */
 int fn2b200_correlation_forward_cat(const float *input1, const float *input2, float *cat, int cat_channels,
                                     int ch_offset, float leaky_slope, int B, int C, int H, int W, int pad_size,
@@ -102,9 +105,10 @@ int fn2b200_correlation_forward_cat(const float *input1, const float *input2, fl
                                     int corr_type_multiply, void *workspace, size_t workspace_bytes, void *stream);
 
 /*
- * Tensor-core backward, same workspace size and layout as the forward's.  workspace_has_split != 0
- * promises that the workspace still holds what fn2b200_correlation_forward_ws wrote for the SAME
- * input1/input2 (the split pass is then skipped).  FN2B200_CORR_BWD=fma forces the FMA kernels.
+ * fn2b200_correlation_backward_workspace() returns the workspace bytes of the tensor-core backward (same size and
+ * layout as the forward's; 0 = FP32-FMA kernels, also under FN2B200_CORR_BWD=fma).  fn2b200_correlation_backward_ws()
+ * equals fn2b200_correlation_backward_cat with cat_channels = D, ch_offset = 0, leaky_slope = 1 (cat unused):
+ * grad_output [B,D,oH,oW].
  */
 size_t fn2b200_correlation_backward_workspace(int B, int C, int H, int W, int pad_size, int kernel_size,
                                               int max_displacement, int stride1, int stride2);
@@ -115,18 +119,22 @@ int fn2b200_correlation_backward_ws(const float *input1, const float *input2, co
                                     size_t workspace_bytes, int workspace_has_split, void *stream);
 
 /*
- * Backward of fn2b200_correlation_forward_cat: the input gradients of
+ * The correlation backward: the input gradients of
  *     cat[:, ch_offset : ch_offset + D] = LeakyReLU(leaky_slope)(correlation(input1, input2))
  * given grad_cat, the gradient of the whole [B, cat_channels, oH, oW] concat buffer, and `cat`, the buffer the forward
  * wrote (same layout; only its [ch_offset, ch_offset + D) channels are read).  Every gradOutput value is
  *     gO[n,d,p] = grad_cat[n, ch_offset+d, p] * (cat[n, ch_offset+d, p] > 0 ? 1 : leaky_slope)
  * (LeakyReLU's derivative read from its output, as torch's in-place LeakyReLU does), applied per element before any
- * other arithmetic, so the result is bit-identical to fn2b200_correlation_backward_ws on that masked, dense gO.  The
- * slice is read in place: no masked copy of the cost volume is written, and the tensor-core path stays one launch.
- * leaky_slope = 1: no activation (cat may be NULL); leaky_slope < 0 -> FN2B200_EINVAL (the output's sign no longer gives
- * the mask).  Workspace as in fn2b200_correlation_backward_ws (NULL -> FP32-FMA kernels; FN2B200_CORR_BWD=fma honoured).
- * Channel range outside the buffer or a buffer of 2^31 elements or more -> FN2B200_EINVAL; stride1 != 1 ->
- * FN2B200_EUNSUPPORTED; B == 0 is a no-op.
+ * other arithmetic, so the result is bit-identical to the plain backward on that masked, dense gO.  The slice is read in
+ * place: no masked copy of the cost volume is written, and the tensor-core path stays one launch.  leaky_slope = 1: no
+ * activation (cat may be NULL).  grad_input1, grad_input2: [B,C,H,W]; either may be NULL to skip it (both NULL: no-op).
+ * Workspace as in fn2b200_correlation_forward_cat (FN2B200_CORR_BWD=fma forces the FP32-FMA kernels);
+ * workspace_has_split != 0 promises that it still holds what the forward wrote for the SAME input1/input2 (the split
+ * pass is then skipped).
+ * leaky_slope < 0 (the output's sign no longer gives the mask), bad shape or parameters, a channel range outside the
+ * buffer or a tensor of 2^31 elements or more -> FN2B200_EINVAL; stride1 != 1 -> FN2B200_EUNSUPPORTED (the reference's
+ * backward indexes out of bounds, correlation_cuda_kernel.cu:163-164 vs :520); NULL input1, input2, grad_cat, or cat
+ * with leaky_slope != 1 -> FN2B200_ENULL; B == 0 is a no-op.
  */
 int fn2b200_correlation_backward_cat(const float *input1, const float *input2, const float *grad_cat, const float *cat,
                                      int cat_channels, int ch_offset, float leaky_slope, float *grad_input1,
@@ -135,9 +143,8 @@ int fn2b200_correlation_backward_cat(const float *input1, const float *input2, c
                                      void *workspace, size_t workspace_bytes, int workspace_has_split, void *stream);
 
 /*
- * grad_output: [B,D,oH,oW]; grad_input1, grad_input2: [B,C,H,W] (either may be NULL to skip it).
- * stride1 must be 1 (the reference's backward indexes out of bounds otherwise,
- * correlation_cuda_kernel.cu:163-164 vs :520) -> FN2B200_EUNSUPPORTED.
+ * fn2b200_correlation_backward_cat with cat_channels = D, ch_offset = 0, leaky_slope = 1 and no workspace (FP32-FMA
+ * kernels): grad_output [B,D,oH,oW].
  */
 int fn2b200_correlation_backward(const float *input1, const float *input2,
                                  const float *grad_output, float *grad_input1,
@@ -248,10 +255,11 @@ int fn2b200_channelnorm_backward_16(const void *input1, const void *output, cons
                                     void *stream);
 
 /*
- * Introspection for benchmarks/tests: which kernel family the correlation entry points would
- * dispatch to for these parameters.  0 = generic gather kernels, 1 = TMA-tiled FP32-FMA kernels,
- * 2 = tensor cores (wgmma) for forward AND backward when a workspace is supplied through the *_ws
- * entry points (FN2B200_CORR_FWD=fma / FN2B200_CORR_BWD=fma select family 1 for that direction).
+ * Introspection for benchmarks/tests: the kernel family a correlation forward runs for these parameters, given 16-byte
+ * aligned pointers and a large-enough workspace (FN2B200_CORR_FWD honoured).  0 = generic gather kernels, 1 = TMA-tiled
+ * FP32-FMA kernels, 2 = tensor cores (wgmma).  The backward follows the same rule with FN2B200_CORR_BWD.  A call
+ * without the workspace cannot run family 2, one with misaligned pointers not family 1; it then runs the next family
+ * whose conditions hold.  -1: invalid parameters.
  */
 int fn2b200_correlation_path(int C, int H, int W, int pad_size, int kernel_size,
                              int max_displacement, int stride1, int stride2);

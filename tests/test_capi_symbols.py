@@ -65,7 +65,7 @@ def test_out_shape_and_path_queries():
     from flownet2_b200._lib import LIB
     assert F2.correlation_out_shape(256, 48, 64, 20, 1, 20, 1, 2) == (441, 48, 64)
     assert F2.correlation_out_shape(8, 12, 13, 2, 1, 4, 2, 2) == (25, 4, 5)
-    assert LIB.fn2b200_correlation_path(256, 112, 256, 20, 1, 20, 1, 2) == 2   # FlowNetC -> tensor-core fwd + tiled bwd
+    assert LIB.fn2b200_correlation_path(256, 112, 256, 20, 1, 20, 1, 2) == 2   # FlowNetC -> tensor cores, forward and backward
     assert LIB.fn2b200_correlation_path(20, 112, 256, 20, 1, 20, 1, 2) == 1    # C % 64 != 0 -> TMA-tiled FMA kernels
     assert LIB.fn2b200_correlation_path(256, 111, 256, 20, 1, 20, 1, 2) == 1   # odd H -> FMA kernels
     assert LIB.fn2b200_correlation_forward_workspace(8, 256, 112, 256, 20, 1, 20, 1, 2) == 8 * 8 * 256 * 112 * 256
