@@ -65,6 +65,12 @@ def _load():
     lib.fn2b200_warp_concat_backward.argtypes = ([_c_ptr, lp, _c_int, _c_ptr, _c_ptr] + [_c_int] * 5 + [ctypes.c_float] + [_c_int] * 2
                                                  + [_c_ptr, _c_ptr, _c_ptr, ctypes.c_size_t] + [_c_int] * 3 + [_c_ptr])
     lib.fn2b200_warp_concat_backward.restype = _c_int
+    lib.fn2b200_warp_concat_backward_up_workspace.argtypes = [_c_int] * 6
+    lib.fn2b200_warp_concat_backward_up_workspace.restype = ctypes.c_size_t
+    lib.fn2b200_warp_concat_backward_up.argtypes = ([_c_ptr, lp, _c_int, _c_ptr, _c_int, _c_int, _c_int, ctypes.c_float, _c_ptr]
+                                                    + [_c_int] * 5 + [ctypes.c_float] + [_c_int] * 2
+                                                    + [_c_ptr, _c_ptr, _c_ptr, ctypes.c_size_t] + [_c_int] * 3 + [_c_ptr])
+    lib.fn2b200_warp_concat_backward_up.restype = _c_int
     lib.fn2b200_resample2d_backward.argtypes = [_c_ptr, lp, _c_ptr, _c_ptr, _c_ptr, _c_ptr] + [_c_int] * 9 + [_c_ptr]
     lib.fn2b200_resample2d_backward_workspace.argtypes = [lp] + [_c_int] * 6
     lib.fn2b200_resample2d_backward_workspace.restype = ctypes.c_size_t
@@ -96,6 +102,7 @@ SYMBOLS = (
     "fn2b200_resample2d_forward", "fn2b200_resample2d_backward",
     "fn2b200_resample2d_forward_up", "fn2b200_warp_concat_forward",
     "fn2b200_warp_concat_backward_workspace", "fn2b200_warp_concat_backward",
+    "fn2b200_warp_concat_backward_up_workspace", "fn2b200_warp_concat_backward_up",
     "fn2b200_resample2d_backward_workspace", "fn2b200_resample2d_backward_ws",
     "fn2b200_channelnorm_forward", "fn2b200_channelnorm_backward",
     "fn2b200_channelnorm_forward_16", "fn2b200_channelnorm_backward_16",

@@ -352,29 +352,62 @@ int fn2b200_resample2d_backward(const float *img, const int64_t *istride, const 
 }
 
 size_t fn2b200_warp_concat_backward_workspace(int B, int C, int H, int W) {
-    if (B <= 0 || C < 1 || C > 3 || H <= 0 || W <= 0) return 0;
-    return resample2d_backward_workspace_bytes(B, H, W);
+    return fn2b200_warp_concat_backward_up_workspace(B, C, H, W, 0, 1);
+}
+
+size_t fn2b200_warp_concat_backward_up_workspace(int B, int C, int H, int W, int upsample_mode, int need_x) {
+    if (B <= 0 || C < 1 || C > 3 || H <= 0 || W <= 0 || upsample_mode < 0 || upsample_mode > 2) return 0;
+    return warp_concat_backward_workspace_bytes(B, H, W, upsample_mode, need_x != 0);
+}
+
+// The two backward entry points: `plain` is fn2b200_warp_concat_backward (full-resolution flow, both gradients
+// required, its own message prefix and workspace query); otherwise fn2b200_warp_concat_backward_up.
+static int warp_concat_backward(bool plain, const float *x, const int64_t *xstride, int C, const float *flow, int fh,
+                                int fw, int upsample_mode, float flow_mul, const float *grad_cat, int cat_channels,
+                                int ch_x, int n_x, int ch_warped, int ch_flow, float flow_div, int ch_flow_norm,
+                                int ch_diff_norm, float *grad_x, float *grad_flow, void *workspace, size_t workspace_bytes,
+                                int B, int H, int W, void *stream) {
+    const char *who = plain ? "warp_concat_backward" : "warp_concat_backward_up";
+    if (B < 0 || C < 1 || H <= 0 || W <= 0 || cat_channels < 1)
+        return fail(FN2B200_EINVAL, "%s: bad shape B=%d C=%d H=%d W=%d cat_channels=%d", who, B, C, H, W, cat_channels);
+    if (C > 3) return fail(FN2B200_EUNSUPPORTED, "%s: C=%d > 3 (the interleaved gradient scratch holds 4 floats per pixel)", who, C);
+    if (!xstride) return fail(FN2B200_ENULL, "%s: null stride array", who);
+    int rc = plain ? 0 : check_flow_src(who, flow, fh, fw, upsample_mode, H, W);
+    if (rc) return rc;
+    if ((rc = check_warp_layout(who, C, cat_channels, ch_x, n_x, ch_warped, ch_flow, flow_div, ch_flow_norm, ch_diff_norm)))
+        return rc;
+    if ((int64_t)B * cat_channels * H * W >= (1LL << 31)) return fail(FN2B200_EINVAL, "%s: tensor exceeds 2^31 elements", who);
+    if (B == 0) return 0;
+    if (plain ? (!x || !flow || !grad_cat || !grad_x || !grad_flow) : (grad_x || grad_flow) && (!x || !grad_cat))
+        return fail(FN2B200_ENULL, "%s: null pointer", who);
+    if (!grad_x && !grad_flow) return 0;          // no gradient wanted
+    const size_t need = warp_concat_backward_workspace_bytes(B, H, W, upsample_mode, grad_x != nullptr);
+    if ((need && !workspace) || workspace_bytes < need || (reinterpret_cast<uintptr_t>(workspace) & 15))
+        return fail(FN2B200_EINVAL, "%s: needs a 16-byte aligned workspace of fn2b200_%s_workspace() bytes", who, who);
+    if ((rc = bind_device_of(flow))) return rc;
+    const FlowSrc fs = {flow, fh, fw, upsample_mode, upsample_mode ? flow_mul : 1.f};
+    WarpOut o = {nullptr, cat_channels, ch_x, n_x, ch_warped, ch_flow, ch_flow_norm, ch_diff_norm, flow_div};
+    return warp_concat_backward_tile(x, xstride, fs, grad_cat, o, grad_x, grad_flow, workspace, B, C, H, W,
+                                     (cudaStream_t)stream);
 }
 
 int fn2b200_warp_concat_backward(const float *x, const int64_t *xstride, int C, const float *flow, const float *grad_cat,
                                  int cat_channels, int ch_x, int n_x, int ch_warped, int ch_flow, float flow_div,
                                  int ch_flow_norm, int ch_diff_norm, float *grad_x, float *grad_flow, void *workspace,
                                  size_t workspace_bytes, int B, int H, int W, void *stream) {
-    if (B < 0 || C < 1 || H <= 0 || W <= 0 || cat_channels < 1)
-        return fail(FN2B200_EINVAL, "warp_concat_backward: bad shape B=%d C=%d H=%d W=%d cat_channels=%d", B, C, H, W, cat_channels);
-    if (C > 3) return fail(FN2B200_EUNSUPPORTED, "warp_concat_backward: C=%d > 3 (the interleaved gradient scratch holds 4 floats per pixel)", C);
-    if (!xstride) return fail(FN2B200_ENULL, "warp_concat_backward: null stride array");
-    int rc = check_warp_layout("warp_concat_backward", C, cat_channels, ch_x, n_x, ch_warped, ch_flow, flow_div, ch_flow_norm,
-                               ch_diff_norm);
-    if (rc) return rc;
-    if ((int64_t)B * cat_channels * H * W >= (1LL << 31)) return fail(FN2B200_EINVAL, "warp_concat_backward: tensor exceeds 2^31 elements");
-    if (B == 0) return 0;
-    if (!x || !flow || !grad_cat || !grad_x || !grad_flow) return fail(FN2B200_ENULL, "warp_concat_backward: null pointer");
-    if (!workspace || workspace_bytes < resample2d_backward_workspace_bytes(B, H, W) || (reinterpret_cast<uintptr_t>(workspace) & 15))
-        return fail(FN2B200_EINVAL, "warp_concat_backward: needs a 16-byte aligned workspace of fn2b200_warp_concat_backward_workspace() bytes");
-    if ((rc = bind_device_of(flow))) return rc;
-    WarpOut o = {nullptr, cat_channels, ch_x, n_x, ch_warped, ch_flow, ch_flow_norm, ch_diff_norm, flow_div};
-    return warp_concat_backward_tile(x, xstride, flow, grad_cat, o, grad_x, grad_flow, workspace, B, C, H, W, (cudaStream_t)stream);
+    return warp_concat_backward(true, x, xstride, C, flow, H, W, 0, 1.f, grad_cat, cat_channels, ch_x, n_x, ch_warped,
+                                ch_flow, flow_div, ch_flow_norm, ch_diff_norm, grad_x, grad_flow, workspace,
+                                workspace_bytes, B, H, W, stream);
+}
+
+int fn2b200_warp_concat_backward_up(const float *x, const int64_t *xstride, int C, const float *flow, int fh, int fw,
+                                    int upsample_mode, float flow_mul, const float *grad_cat, int cat_channels, int ch_x,
+                                    int n_x, int ch_warped, int ch_flow, float flow_div, int ch_flow_norm,
+                                    int ch_diff_norm, float *grad_x, float *grad_flow, void *workspace,
+                                    size_t workspace_bytes, int B, int H, int W, void *stream) {
+    return warp_concat_backward(false, x, xstride, C, flow, fh, fw, upsample_mode, flow_mul, grad_cat, cat_channels, ch_x,
+                                n_x, ch_warped, ch_flow, flow_div, ch_flow_norm, ch_diff_norm, grad_x, grad_flow,
+                                workspace, workspace_bytes, B, H, W, stream);
 }
 
 size_t fn2b200_resample2d_backward_workspace(const int64_t *istride, int B, int C, int iH, int iW, int H, int W) {

@@ -166,8 +166,12 @@ int resample2d_backward_tile(const float *img, const int64_t *istride, const flo
 size_t resample2d_backward_workspace_bytes(int B, int iH, int iW);
 int resample2d_backward_finish(const float *T, float *gimg, int accumulate, int B, int C, int iH, int iW, cudaStream_t st,
                                long gimg_bstride = 0);
-// backward of the fused warp -> diff -> channel-norm -> concat forward (full-resolution flow, C <= 3); workspace as above
-int warp_concat_backward_tile(const float *x, const int64_t *xstride, const float *flow, const float *gcat, const WarpOut &o,
+// backward of the fused upsample -> warp -> diff -> channel-norm -> concat forward (C <= 3).  gx == NULL: no image
+// gradient (no scatter); gflow == NULL: no flow gradient.  gflow is [B,2,fs.fh,fs.fw].  workspace: the scatter scratch
+// above when gx is wanted, followed by the bilinear adjoint's per-tile partials (fs.mode == 1):
+// warp_concat_backward_workspace_bytes() in all.
+size_t warp_concat_backward_workspace_bytes(int B, int H, int W, int upsample_mode, bool need_x);
+int warp_concat_backward_tile(const float *x, const int64_t *xstride, const FlowSrc &fs, const float *gcat, const WarpOut &o,
                               float *gx, float *gflow, void *workspace, int B, int C, int H, int W, cudaStream_t st);
 
 struct CorrParams {

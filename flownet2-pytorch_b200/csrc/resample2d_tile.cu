@@ -215,36 +215,63 @@ resample2d_bwd_tile(ImgView im, FlowSrc fs, const float *__restrict__ gout, floa
 }
 
 // ---------------------------------------------------------------------------------------------------------------
-// Backward of the fused warp -> diff -> channel-norm -> concat forward (full-resolution flow; in a training graph the
-// x4 upsample stays a torch module in front of it).  Per pixel, with v = the warped img1 (recomputed from the taps the
-// flow gradient needs anyway), d = img0 - v, n = |d|, f = |flow|:
+// Backward of the fused upsample -> warp -> diff -> channel-norm -> concat forward.  Per pixel, with flow = the
+// full-resolution flow (recomputed by load_flow exactly as the forward does), v = the warped img1 (recomputed from the
+// taps the flow gradient needs anyway), d = img0 - v, n = |d|, f = |flow|:
 //   g_d[c]   = gcat[ch_dnorm] * d[c] / (n + 1e-9)                      ChannelNorm backward, channelnorm_kernel.cu:92
 //   g_v[c]   = gcat[ch_warped + c] - g_d[c]                            the subtraction (models.py:134)
 //   gx[c]    = gcat[ch_x + c] + g_d[c]          (img0 half),   gx[C + c] = gcat[ch_x + C + c] + scatter of g_v (K6)
-//   gflow    = K7(g_v) + gcat[ch_flow ..] / flow_div + gcat[ch_fnorm] * flow / (f + 1e-9)
+//   g_up     = K7(g_v) + gcat[ch_flow ..] / flow_div + gcat[ch_fnorm] * flow / (f + 1e-9)
 // The scatter goes through the interleaved scratch T exactly as in resample2d_bwd_tile<.., 2>; the finishing kernel adds
 // T to the direct term this kernel stores into gx[:, C:2C].
+// UP selects where the flow comes from and where g_up goes (FlowSrc mode):
+//   0  full-resolution flow: g_up is the flow gradient, stored to gflow [B,2,H,W]
+//   2  nearest x4: g_up is staged in shared memory; the 32 x 8 PY tile is aligned to 4, so each 4 x 4 block of it is one
+//      quarter-resolution cell, summed in a fixed order, times mul, and stored to gflow [B,2,fh,fw]
+//   1  bilinear x4: a cell receives from full-resolution rows / columns [4i - 2, 4i + 5], so the cells of a tile edge
+//      are shared with the neighbouring tiles.  The tile's g_up is reduced in shared memory (rows of pixels onto cell
+//      columns, then pixel rows onto cell rows, with load_flow's own lambdas; fixed order) into (8 PY / 4 + 2) x 10
+//      per-tile partials per component, written to gflow = the partial scratch; warp_concat_up_finish adds the <= 2 x 2
+//      partials of each cell in a fixed order.  Deterministic: no atomics touch the flow gradient.
+// NX / NF: the image / flow gradient is wanted (gx / gflow are not touched otherwise): without NX there is no K6
+// scatter, without NF no K7 and no flow reduction.
 // ---------------------------------------------------------------------------------------------------------------
-template <int CT, int PY>
+// weight of full-resolution pixel p in quarter-resolution cell `cell` of load_flow's bilinear x4 upsample (n cells)
+__device__ __forceinline__ float up4_weight(int p, int cell, int n) {
+    const float s = fmaxf(0.25f * ((float)p + 0.5f) - 0.5f, 0.f);
+    const int i1 = (int)s, ip = i1 < n - 1 ? 1 : 0;
+    const float l1 = s - (float)i1;
+    return (i1 == cell ? 1.f - l1 : 0.f) + (i1 + ip == cell ? l1 : 0.f);
+}
+
+template <int CT, int PY, int UP, bool NX, bool NF>
 __global__ void __launch_bounds__(256)
 warp_concat_bwd_tile(ImgView xv, FlowSrc fs, const float *__restrict__ gcat, WarpOut o, float *__restrict__ gx,
                      float *__restrict__ T, float *__restrict__ gflow, int H, int W, int tiles_x, int tiles_y) {
+    constexpr int TH = 8 * PY, NR = TH / 4 + 2, NC = 32 / 4 + 2;          // tile rows; bilinear partial cells
+    constexpr bool STAGE = UP != 0 && NF;
+    __shared__ float sg[STAGE ? 2 : 1][STAGE ? TH : 1][32];                 // g_up of the tile (0 outside the image)
+    __shared__ float sr[UP == 1 && NF ? 2 : 1][UP == 1 && NF ? TH : 1][NC];  // bilinear: pixel rows x cell columns
     const int tid = threadIdx.x, lx = tid & 31, ly = tid >> 5;
     int t = blockIdx.x;
     const int bxi = t % tiles_x;
     t /= tiles_x;
     const int byi = t % tiles_y, b = t / tiles_y;
     const int x = bxi * 32 + lx, y0 = byi * (8 * PY) + ly;
-    if (x >= W) return;
+    if (UP == 0 && x >= W) return;
     const long hw = (long)H * W;
     const float *i0 = xv.p + (long)b * xv.sb, *i1 = i0 + CT * xv.sc;
     const float *gc = gcat + (long)b * o.cat_channels * hw;
-    float *gxb = gx + (long)b * 2 * CT * hw;
-    float *Tb = T + (long)b * hw * 4;
+    float *gxb = NX ? gx + (long)b * 2 * CT * hw : nullptr;
+    float *Tb = NX ? T + (long)b * hw * 4 : nullptr;
+    if (STAGE) {
+#pragma unroll
+        for (int j = 0; j < PY; ++j) sg[0][ly + 8 * j][lx] = sg[1][ly + 8 * j][lx] = 0.f;
+    }
 #pragma unroll
     for (int j = 0; j < PY; ++j) {
         const int y = y0 + 8 * j;
-        if (y >= H) continue;
+        if (y >= H || (UP != 0 && x >= W)) continue;
         const long pix = (long)y * W + x;
         const float2 fl = load_flow(fs, b, y, x, H, W);
         const float xf = (float)x + fl.x, yf = (float)y + fl.y;
@@ -276,23 +303,30 @@ warp_concat_bwd_tile(ImgView xv, FlowSrc fs, const float *__restrict__ gcat, War
             const float gd = o.ch_dnorm >= 0 ? gn * d[c] / (nrm + 1e-9f) : 0.f;
             const float gw = o.ch_warped >= 0 ? ldg_stream1(gc + (long)(o.ch_warped + c) * hw + pix) : 0.f;
             gv[c] = gw - gd;
-            const float gx0 = (o.ch_x >= 0 && c < o.n_x) ? ldg_stream1(gc + (long)(o.ch_x + c) * hw + pix) : 0.f;
-            const float gx1 = (o.ch_x >= 0 && CT + c < o.n_x) ? ldg_stream1(gc + (long)(o.ch_x + CT + c) * hw + pix) : 0.f;
-            __stcs(gxb + (long)c * hw + pix, gx0 + gd);
-            __stcs(gxb + (long)(CT + c) * hw + pix, gx1);          // + the scattered part, added by the finishing kernel
-            // K7: d/dxf with gamma = 1 - beta (:181-192), d/dyf with gamma = 1 - alpha (:168-179)
-            gfx += gv[c] * ((1.f - be) * (iTR[c] - iTL[c]) + be * (iBR[c] - iBL[c]));
-            gfy += gv[c] * ((1.f - al) * (iBL[c] - iTL[c]) + al * (iBR[c] - iTR[c]));
+            if (NX) {
+                const float gx0 = (o.ch_x >= 0 && c < o.n_x) ? ldg_stream1(gc + (long)(o.ch_x + c) * hw + pix) : 0.f;
+                const float gx1 = (o.ch_x >= 0 && CT + c < o.n_x) ? ldg_stream1(gc + (long)(o.ch_x + CT + c) * hw + pix) : 0.f;
+                __stcs(gxb + (long)c * hw + pix, gx0 + gd);
+                __stcs(gxb + (long)(CT + c) * hw + pix, gx1);          // + the scattered part, added by the finishing kernel
+            }
+            if (NF) {
+                // K7: d/dxf with gamma = 1 - beta (:181-192), d/dyf with gamma = 1 - alpha (:168-179)
+                gfx += gv[c] * ((1.f - be) * (iTR[c] - iTL[c]) + be * (iBR[c] - iBL[c]));
+                gfy += gv[c] * ((1.f - al) * (iBL[c] - iTL[c]) + al * (iBR[c] - iTR[c]));
+            }
         }
-        // K6: image-gradient scatter, int()-truncation fractions (:105-114); image dims == flow dims here
-        const float at = xf - (float)(int)xf, bt = yf - (float)(int)yf;
-        const float s00 = (1.f - at) * (1.f - bt), s01 = at * (1.f - bt), s10 = (1.f - at) * bt, s11 = at * bt;
-        float *pTL = Tb + ((long)tp.yT * W + tp.xL) * 4, *pTR = Tb + ((long)tp.yT * W + tp.xR) * 4;
-        float *pBL = Tb + ((long)tp.yB * W + tp.xL) * 4, *pBR = Tb + ((long)tp.yB * W + tp.xR) * 4;
-        red_add_v4(pTL, s00 * gv[0], s00 * gv[1], s00 * gv[2], 0.f);
-        red_add_v4(pTR, s01 * gv[0], s01 * gv[1], s01 * gv[2], 0.f);
-        red_add_v4(pBL, s10 * gv[0], s10 * gv[1], s10 * gv[2], 0.f);
-        red_add_v4(pBR, s11 * gv[0], s11 * gv[1], s11 * gv[2], 0.f);
+        if (NX) {
+            // K6: image-gradient scatter, int()-truncation fractions (:105-114); image dims == flow dims here
+            const float at = xf - (float)(int)xf, bt = yf - (float)(int)yf;
+            const float s00 = (1.f - at) * (1.f - bt), s01 = at * (1.f - bt), s10 = (1.f - at) * bt, s11 = at * bt;
+            float *pTL = Tb + ((long)tp.yT * W + tp.xL) * 4, *pTR = Tb + ((long)tp.yT * W + tp.xR) * 4;
+            float *pBL = Tb + ((long)tp.yB * W + tp.xL) * 4, *pBR = Tb + ((long)tp.yB * W + tp.xR) * 4;
+            red_add_v4(pTL, s00 * gv[0], s00 * gv[1], s00 * gv[2], 0.f);
+            red_add_v4(pTR, s01 * gv[0], s01 * gv[1], s01 * gv[2], 0.f);
+            red_add_v4(pBL, s10 * gv[0], s10 * gv[1], s10 * gv[2], 0.f);
+            red_add_v4(pBR, s11 * gv[0], s11 * gv[1], s11 * gv[2], 0.f);
+        }
+        if (!NF) continue;
         if (o.ch_flow >= 0) {
             gfx += ldg_stream1(gc + (long)o.ch_flow * hw + pix) / o.flow_div;
             gfy += ldg_stream1(gc + (long)(o.ch_flow + 1) * hw + pix) / o.flow_div;
@@ -303,10 +337,74 @@ warp_concat_bwd_tile(ImgView xv, FlowSrc fs, const float *__restrict__ gcat, War
             gfx += gf * fl.x / (fnrm + 1e-9f);
             gfy += gf * fl.y / (fnrm + 1e-9f);
         }
+        if (STAGE) {
+            sg[0][ly + 8 * j][lx] = gfx;
+            sg[1][ly + 8 * j][lx] = gfy;
+            continue;
+        }
         float *gfp = gflow + (long)b * 2 * hw + pix;
         __stcs(gfp, gfx);
         __stcs(gfp + hw, gfy);
     }
+    if (!STAGE) return;
+    // ---- adjoint of the x4 upsample (no thread has left: the early return above is UP == 0 only) ----
+    __syncthreads();
+    if (UP == 2) {
+        constexpr int NCELL = (TH / 4) * 8;
+        if (tid < 2 * NCELL) {
+            const int comp = tid / NCELL, r = (tid % NCELL) >> 3, q = tid & 7;
+            const int ci = byi * (TH / 4) + r, cj = bxi * 8 + q;
+            if (ci < fs.fh && cj < fs.fw) {
+                float s = 0.f;
+#pragma unroll
+                for (int yy = 0; yy < 4; ++yy)
+#pragma unroll
+                    for (int xx = 0; xx < 4; ++xx) s += sg[comp][4 * r + yy][4 * q + xx];
+                __stcs(gflow + ((long)b * 2 + comp) * fs.fh * fs.fw + (long)ci * fs.fw + cj, __fmul_rn(s, fs.mul));
+            }
+        }
+        return;
+    }
+    // bilinear: tile-local cell (r, q) is cell (TH/4 byi - 1 + r, 8 bxi - 1 + q); its pixels are local rows / columns
+    // [4r - 6, 4r + 1] / [4q - 6, 4q + 1] clipped to the tile
+    for (int it = tid; it < 2 * TH * NC; it += 256) {
+        const int comp = it / (TH * NC), yl = (it / NC) % TH, q = it % NC;
+        const int cj = bxi * 8 - 1 + q, xhi = min(4 * q + 1, 31);
+        float s = 0.f;
+        for (int xl = max(4 * q - 6, 0); xl <= xhi; ++xl) s = __fmaf_rn(up4_weight(bxi * 32 + xl, cj, fs.fw), sg[comp][yl][xl], s);
+        sr[comp][yl][q] = s;
+    }
+    __syncthreads();
+    if (tid < 2 * NR * NC) {
+        const int comp = tid / (NR * NC), r = (tid / NC) % NR, q = tid % NC;
+        const int ci = byi * (TH / 4) - 1 + r, yhi = min(4 * r + 1, TH - 1);
+        float s = 0.f;
+        for (int yl = max(4 * r - 6, 0); yl <= yhi; ++yl) s = __fmaf_rn(up4_weight(byi * TH + yl, ci, fs.fh), sr[comp][yl][q], s);
+        gflow[(long)blockIdx.x * (2 * NR * NC) + tid] = s;
+    }
+}
+
+// Bilinear x4 flow gradient from the per-tile partials of warp_concat_bwd_tile<.., 1, .., true>: cell (i, j) of
+// component c sums the partials of the tiles (ty, tx) whose (TR + 2) x (TC + 2) cell window holds it -- ty ascending,
+// then tx -- and multiplies by mul.  TR x TC: the cells one tile covers (4 x 8 for a 16 x 32 pixel tile).
+template <int TR, int TC>
+__global__ void __launch_bounds__(256)
+warp_concat_up_finish(const float *__restrict__ P, float *__restrict__ gflow, int fh, int fw, int tiles_x, int tiles_y,
+                      float mul, long n) {
+    constexpr int NR = TR + 2, NC = TC + 2;
+    const long idx = (long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (idx >= n) return;
+    const int j = (int)(idx % fw), i = (int)((idx / fw) % fh);
+    const long bc = idx / ((long)fh * fw);
+    const int comp = (int)(bc & 1), b = (int)(bc >> 1);
+    const int ty0 = max((i + TR - 1) / TR - 1, 0), ty1 = min((i + 1) / TR, tiles_y - 1);
+    const int tx0 = max((j + TC - 1) / TC - 1, 0), tx1 = min((j + 1) / TC, tiles_x - 1);
+    float s = 0.f;
+    for (int ty = ty0; ty <= ty1; ++ty)
+        for (int tx = tx0; tx <= tx1; ++tx)
+            s += __ldg(P + (((long)b * tiles_y + ty) * tiles_x + tx) * (2 * NR * NC) + (comp * NR + i - TR * ty + 1) * NC +
+                       j - TC * tx + 1);
+    __stcs(gflow + idx, __fmul_rn(s, mul));
 }
 
 // T[b][y][x][4] -> gimg[b][c][y][x] (accumulate != 0: added to what gimg holds -- the *_cuda shim's caller-zeroed buffer)
@@ -433,24 +531,58 @@ int resample2d_backward_finish(const float *T, float *gimg, int accumulate, int 
     return check_launch("resample2d_backward (finish)");
 }
 
-int warp_concat_backward_tile(const float *x, const int64_t *xs, const float *flow, const float *gcat, const WarpOut &o,
+// PY = 2: 16 live tap registers per channel set; a 32 x 16 pixel tile, 8 x 4 quarter-resolution cells
+static long warp_concat_tiles(int B, int H, int W) { return (long)((W + 31) / 32) * ((H + 15) / 16) * B; }
+
+size_t warp_concat_backward_workspace_bytes(int B, int H, int W, int upsample_mode, bool need_x) {
+    return (need_x ? resample2d_backward_workspace_bytes(B, H, W) : 0) +
+           (upsample_mode == 1 ? (size_t)warp_concat_tiles(B, H, W) * 2 * (4 + 2) * (8 + 2) * sizeof(float) : 0);
+}
+
+int warp_concat_backward_tile(const float *x, const int64_t *xs, const FlowSrc &fs, const float *gcat, const WarpOut &o,
                               float *gx, float *gflow, void *workspace, int B, int C, int H, int W, cudaStream_t st) {
-    const int tiles_x = (W + 31) / 32, tiles_y = (H + 15) / 16;          // PY = 2: 16 live tap registers per channel set
-    const long ntiles = (long)tiles_x * tiles_y * B;
+    const int tiles_x = (W + 31) / 32, tiles_y = (H + 15) / 16;
+    const long ntiles = warp_concat_tiles(B, H, W);
     if (ntiles >= (1L << 31)) return fail(FN2B200_EINVAL, "warp_concat_backward: %ld tiles exceed the grid limit", ntiles);
-    float *T = static_cast<float *>(workspace);
-    cudaError_t e = cudaMemsetAsync(T, 0, resample2d_backward_workspace_bytes(B, H, W), st);
-    if (e != cudaSuccess) return fail((int)e, "warp_concat_backward: workspace memset failed (%s)", cudaGetErrorString(e));
-    const ImgView v = view_of(x, xs);
-    const FlowSrc fs = {flow, H, W, 0, 1.f};
-    const unsigned grid = (unsigned)ntiles;
-    switch (C) {
-        case 1: warp_concat_bwd_tile<1, 2><<<grid, 256, 0, st>>>(v, fs, gcat, o, gx, T, gflow, H, W, tiles_x, tiles_y); break;
-        case 2: warp_concat_bwd_tile<2, 2><<<grid, 256, 0, st>>>(v, fs, gcat, o, gx, T, gflow, H, W, tiles_x, tiles_y); break;
-        default: warp_concat_bwd_tile<3, 2><<<grid, 256, 0, st>>>(v, fs, gcat, o, gx, T, gflow, H, W, tiles_x, tiles_y); break;
+    // workspace: [the scatter scratch T, when gx is wanted][the bilinear per-tile partials, when gflow is wanted]
+    float *T = gx ? static_cast<float *>(workspace) : nullptr;
+    float *P = (fs.mode == 1 && gflow)
+                   ? reinterpret_cast<float *>(static_cast<char *>(workspace) + (gx ? resample2d_backward_workspace_bytes(B, H, W) : 0))
+                   : nullptr;
+    if (T) {
+        cudaError_t e = cudaMemsetAsync(T, 0, resample2d_backward_workspace_bytes(B, H, W), st);
+        if (e != cudaSuccess) return fail((int)e, "warp_concat_backward: workspace memset failed (%s)", cudaGetErrorString(e));
     }
+    const ImgView v = view_of(x, xs);
+    const unsigned grid = (unsigned)ntiles;
+    float *gf = P ? P : gflow;
+#define FN2_WB(CT, UP, NX, NF) warp_concat_bwd_tile<CT, 2, UP, NX, NF><<<grid, 256, 0, st>>>(v, fs, gcat, o, gx, T, gf, H, W, tiles_x, tiles_y)
+#define FN2_WBN(CT, UP)                                                                                                  \
+    do {                                                                                                               \
+        if (gx && gflow) FN2_WB(CT, UP, true, true);                                                                   \
+        else if (gx) FN2_WB(CT, UP, true, false);                                                                      \
+        else FN2_WB(CT, UP, false, true);                                                                              \
+    } while (0)
+#define FN2_WBC(UP)                                                                                                      \
+    switch (C) {                                                                                                       \
+        case 1: FN2_WBN(1, UP); break;                                                                                 \
+        case 2: FN2_WBN(2, UP); break;                                                                                 \
+        default: FN2_WBN(3, UP); break;                                                                                \
+    }
+    if (fs.mode == 1) { FN2_WBC(1) } else if (fs.mode == 2) { FN2_WBC(2) } else { FN2_WBC(0) }
+#undef FN2_WBC
+#undef FN2_WBN
+#undef FN2_WB
     count_launch();
     if (int rc = check_launch("warp_concat_backward")) return rc;
+    if (P) {
+        const long n = (long)B * 2 * fs.fh * fs.fw;
+        warp_concat_up_finish<4, 8><<<(unsigned)((n + 255) / 256), 256, 0, st>>>(P, gflow, fs.fh, fs.fw, tiles_x, tiles_y,
+                                                                                   fs.mul, n);
+        count_launch();
+        if (int rc = check_launch("warp_concat_backward (flow upsample adjoint)")) return rc;
+    }
+    if (!T) return 0;
     // gx[:, C:2C] += T
     return resample2d_backward_finish(T, gx + (long)C * H * W, 1, B, C, H, W, st, (long)2 * C * H * W);
 }

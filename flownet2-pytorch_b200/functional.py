@@ -295,27 +295,36 @@ def warp_concat_forward(x, flow, C=3, upsample=None, flow_mul=1.0, flow_div=1.0,
 
 
 def warp_concat_backward(x, flow, grad_cat, C=3, flow_div=1.0, ch_x=0, n_x=None, ch_warped=None, ch_flow=None,
-                         ch_flow_norm=-1, ch_diff_norm=None):
-    """Backward of warp_concat_forward(x, flow, upsample=None, ...): returns (grad_x [B,2C,H,W], grad_flow [B,2,H,W]).
-    The layout arguments must be the forward's; C <= 3."""
+                         ch_flow_norm=-1, ch_diff_norm=None, upsample=None, flow_mul=1.0, need_x=True, need_flow=True):
+    """Backward of warp_concat_forward(x, flow, upsample=upsample, flow_mul=flow_mul, ...): returns (grad_x [B,2C,H,W],
+    grad_flow shaped like flow -- the quarter-resolution flow's gradient when upsample is "bilinear" / "nearest").  The
+    layout arguments must be the forward's; C <= 3.  need_x / need_flow = False skips that gradient (None is returned
+    for it): without grad_x the kernel does no image-gradient scatter.  grad_flow is bit-identical from run to run and
+    whether or not grad_x is computed."""
     _require_cuda(x, flow, grad_cat)
     xx = x if x.dtype == torch.float32 else x.float()
     fl, gc = _f32c(flow), _f32c(grad_cat)
-    B, _, H, W = fl.shape
-    if tuple(xx.shape[2:]) != (H, W) or xx.size(1) < 2 * C or tuple(gc.shape[2:]) != (H, W) or gc.size(0) != B:
+    mode = UPSAMPLE_MODES[upsample]
+    if fl.dim() != 4 or xx.dim() != 4 or gc.dim() != 4:
+        raise ValueError("warp_concat_backward: expected 4-D x, flow and grad_cat, got %s, %s and %s"
+                         % (tuple(xx.shape), tuple(fl.shape), tuple(gc.shape)))
+    B, _, fh, fw = fl.shape
+    H, W = (fh, fw) if mode == 0 else (4 * fh, 4 * fw)
+    if fl.size(1) != 2 or tuple(xx.shape[2:]) != (H, W) or xx.size(1) < 2 * C or tuple(gc.shape[2:]) != (H, W) or gc.size(0) != B:
         raise ValueError("warp_concat_backward: shapes x %s, flow %s, grad_cat %s do not match" % (tuple(xx.shape), tuple(fl.shape), tuple(gc.shape)))
     n_x = 2 * C if n_x is None else n_x
     ch_warped = 2 * C if ch_warped is None else ch_warped
     ch_flow = 3 * C if ch_flow is None else ch_flow
     ch_diff_norm = 3 * C + 2 if ch_diff_norm is None else ch_diff_norm
     with torch.cuda.device_of(fl):
-        gx = torch.empty((B, 2 * C, H, W), dtype=torch.float32, device=fl.device)
-        gf = torch.empty_like(fl)
-        ws_bytes = int(LIB.fn2b200_warp_concat_backward_workspace(B, C, H, W))
+        gx = torch.empty((B, 2 * C, H, W), dtype=torch.float32, device=fl.device) if need_x else None
+        gf = torch.empty_like(fl) if need_flow else None
+        ws_bytes = int(LIB.fn2b200_warp_concat_backward_up_workspace(B, C, H, W, mode, int(bool(need_x))))
         ws = torch.empty(max(ws_bytes, 16), dtype=torch.uint8, device=fl.device)
-        check(LIB.fn2b200_warp_concat_backward(_ptr(xx), _img_strides(xx), C, _ptr(fl), _ptr(gc), gc.size(1), ch_x, n_x, ch_warped,
-                                               ch_flow, float(flow_div), ch_flow_norm, ch_diff_norm, _ptr(gx), _ptr(gf), _ptr(ws),
-                                               ws_bytes, B, H, W, _stream(fl)), "warp_concat_backward")
+        check(LIB.fn2b200_warp_concat_backward_up(_ptr(xx), _img_strides(xx), C, _ptr(fl), fh, fw, mode, float(flow_mul),
+                                                  _ptr(gc), gc.size(1), ch_x, n_x, ch_warped, ch_flow, float(flow_div),
+                                                  ch_flow_norm, ch_diff_norm, _ptr(gx), _ptr(gf), _ptr(ws), ws_bytes, B, H, W,
+                                                  _stream(fl)), "warp_concat_backward")
     return gx, gf
 
 

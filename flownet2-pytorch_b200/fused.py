@@ -22,9 +22,17 @@ and hyper-parameters are used as they are) and run the same data flow with the g
   separate correlation output kept for backward.  Gradients are bit-identical to the unfused
   ``Correlation`` -> ``LeakyReLU`` -> ``torch.cat`` graph.
 * ``train_forward(net, inputs)`` -- FlowNetC / FlowNet2C with autograd on, through ``CorrelationCat``; returns what
-  ``net.forward`` returns in the net's current mode (flow2..flow6 in training).  FlowNet2 is not covered: its warp
-  groups would need the x4 upsample's backward inside ``warp_concat_backward``.
-* ``WarpConcat`` / ``WarpConcatFunction`` (full-resolution flow, fused forward AND fused backward).
+  ``net.forward`` returns in the net's current mode (flow2..flow6 in training).  FlowNet2 has its own entry point:
+* ``flownet2_train_forward(net, inputs)`` -- FlowNet2 with autograd on: ``CorrelationCat`` in the FlowNetC stage,
+  ``WarpConcat(upsample="bilinear")`` for concat1 / concat2 and ``FusionConcat`` for concat3.  ``flownet2_forward`` is
+  this function under ``torch.no_grad``, so inference and training share one data flow.
+* ``WarpConcat`` / ``WarpConcatFunction`` -- ``upsample -> Resample2d -> diff -> ChannelNorm -> cat`` with a fused
+  forward AND a fused backward.  With ``upsample`` the op takes the quarter-resolution flow2 and its backward returns
+  that flow's gradient directly: the x4 upsample's adjoint runs inside the backward kernel, deterministically (torch's
+  own upsample backward uses atomics), and the full-resolution flow gradient is never written.  The image gradient is
+  only computed when x requires one -- in FlowNet2, x is the normalised input and does not.
+* ``FusionConcat`` / ``FusionConcatFunction`` -- the 11-channel concat3 of the fusion stage from x and the
+  quarter-resolution FlowNetSD / FlowNetS2 flows, same scheme (nearest upsample).
 
 Results agree with the unfused graph to rounding (tests/test_gpu_parity.py::test_fused_forwards_match_unfused_models,
 tests/test_gpu_corr_cat.py).
@@ -36,36 +44,96 @@ from torch.autograd.function import once_differentiable
 from . import functional as F2
 
 
+def _pad_channels(gx, channels):
+    """gx [B, 2C, H, W] -> [B, channels, H, W]: odd trailing channels of x take no part in the op."""
+    if channels > gx.size(1):
+        gx = torch.cat((gx, gx.new_zeros(gx.size(0), channels - gx.size(1), gx.size(2), gx.size(3))), 1)
+    return gx
+
+
 class WarpConcatFunction(Function):
-    """concat1 = cat(x, Resample2d()(x[:, 3:], flow), flow / div_flow, ChannelNorm()(x[:, :3] - warped)) as one
-    differentiable op (models.py:133-138, :145-150); flow is the full-resolution flow (keep nn.Upsample in front of it
-    when training: its backward is torch's).  forward and backward are one kernel each."""
+    """concat1 = cat(x, Resample2d()(x[:, 3:], flow_up), flow_up / div_flow, ChannelNorm()(x[:, :3] - warped)) as one
+    differentiable op (models.py:133-138, :145-150).  upsample=None: flow is the full-resolution flow_up.
+    upsample="bilinear" / "nearest": flow is the quarter-resolution flow2 and flow_up = nn.Upsample(scale_factor=4,
+    mode=upsample)(flow2 * div_flow) (models.py:130, :142) -- folded into the kernels, so the full-resolution flow and
+    its gradient are never materialised.  forward is one kernel; backward one kernel plus the passes that finish the
+    gradients asked for (only those in ctx.needs_input_grad are computed)."""
 
     @staticmethod
-    def forward(ctx, x, flow, div_flow=20.0):
+    def forward(ctx, x, flow, div_flow=20.0, upsample=None):
         ctx.save_for_backward(x, flow)
-        ctx.div_flow = float(div_flow)
-        return F2.warp_concat_forward(x, flow, C=x.size(1) // 2, flow_div=ctx.div_flow)
+        ctx.div_flow, ctx.upsample = float(div_flow), upsample
+        return F2.warp_concat_forward(x, flow, C=x.size(1) // 2, upsample=upsample, flow_mul=ctx.div_flow,
+                                      flow_div=ctx.div_flow)
 
     @staticmethod
     @once_differentiable
     def backward(ctx, grad_cat):
         x, flow = ctx.saved_tensors
-        gx, gf = F2.warp_concat_backward(x, flow, grad_cat, C=x.size(1) // 2, flow_div=ctx.div_flow)
-        if x.size(1) > gx.size(1):           # odd trailing channels of x take no part
-            gx = torch.cat((gx, gx.new_zeros(gx.size(0), x.size(1) - gx.size(1), gx.size(2), gx.size(3))), 1)
-        return (gx if ctx.needs_input_grad[0] else None), (gf if ctx.needs_input_grad[1] else None), None
+        need_x, need_flow = ctx.needs_input_grad[:2]
+        gx, gf = F2.warp_concat_backward(x, flow, grad_cat, C=x.size(1) // 2, flow_div=ctx.div_flow, upsample=ctx.upsample,
+                                         flow_mul=ctx.div_flow, need_x=need_x, need_flow=need_flow)
+        return (_pad_channels(gx, x.size(1)) if need_x else None), gf, None, None
 
 
 class WarpConcat(torch.nn.Module):
-    """nn.Module form of WarpConcatFunction: WarpConcat(div_flow)(x, flow) -> the (3C + 3)-channel concat."""
+    """nn.Module form of WarpConcatFunction: WarpConcat(div_flow, upsample)(x, flow) -> the (3C + 3)-channel concat."""
 
-    def __init__(self, div_flow=20.0):
+    def __init__(self, div_flow=20.0, upsample=None):
         super(WarpConcat, self).__init__()
-        self.div_flow = div_flow
+        self.div_flow, self.upsample = div_flow, upsample
 
     def forward(self, x, flow):
-        return WarpConcatFunction.apply(x, flow, self.div_flow)
+        return WarpConcatFunction.apply(x, flow, self.div_flow, self.upsample)
+
+
+# concat3 of models.py:179: (img0 | sd flow | s2 flow | |sd flow| | |s2 flow| | sd diff norm | s2 diff norm), each flow
+# the nearest x4 upsample of its quarter-resolution flow2 (sd: / div_flow, models.py:167; s2: * div_flow, :154)
+_FUSION_SD = dict(ch_x=0, n_x=3, ch_warped=-1, ch_flow=3, ch_flow_norm=7, ch_diff_norm=9)
+_FUSION_S2 = dict(ch_x=-1, n_x=0, ch_warped=-1, ch_flow=5, ch_flow_norm=8, ch_diff_norm=10)
+
+
+class FusionConcatFunction(Function):
+    """concat3 of models.py:153-179 as one differentiable op: (x [B,6,H,W], sd_flow2, s2_flow2 [B,2,H/4,W/4]) ->
+    [B,11,H,W].  forward = two warp_concat_forward calls into one buffer; backward = two warp_concat_backward calls,
+    each reading its own channels of the concat gradient, the x gradients summed."""
+
+    @staticmethod
+    def forward(ctx, x, sd_flow2, s2_flow2, div_flow=20.0):
+        ctx.save_for_backward(x, sd_flow2, s2_flow2)
+        ctx.div_flow = div = float(div_flow)
+        B, _, H, W = x.shape
+        concat3 = torch.empty((B, 11, H, W), dtype=torch.float32, device=x.device)
+        F2.warp_concat_forward(x, sd_flow2, upsample="nearest", flow_mul=1.0 / div, flow_div=1.0, out=concat3, **_FUSION_SD)
+        F2.warp_concat_forward(x, s2_flow2, upsample="nearest", flow_mul=div, flow_div=1.0, out=concat3, **_FUSION_S2)
+        return concat3
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_cat):
+        x, sd_flow2, s2_flow2 = ctx.saved_tensors
+        need_x, need_sd, need_s2 = ctx.needs_input_grad[:3]
+        div = ctx.div_flow
+        gx = g_sd = g_s2 = None
+        if need_x or need_sd:
+            gx, g_sd = F2.warp_concat_backward(x, sd_flow2, grad_cat, flow_div=1.0, upsample="nearest", flow_mul=1.0 / div,
+                                               need_x=need_x, need_flow=need_sd, **_FUSION_SD)
+        if need_x or need_s2:
+            gx2, g_s2 = F2.warp_concat_backward(x, s2_flow2, grad_cat, flow_div=1.0, upsample="nearest", flow_mul=div,
+                                                need_x=need_x, need_flow=need_s2, **_FUSION_S2)
+            gx = gx2 if gx is None else gx.add_(gx2)
+        return (_pad_channels(gx, x.size(1)) if need_x else None), g_sd, g_s2, None
+
+
+class FusionConcat(torch.nn.Module):
+    """nn.Module form of FusionConcatFunction: FusionConcat(div_flow)(x, sd_flow2, s2_flow2) -> the 11-channel concat3."""
+
+    def __init__(self, div_flow=20.0):
+        super(FusionConcat, self).__init__()
+        self.div_flow = div_flow
+
+    def forward(self, x, sd_flow2, s2_flow2):
+        return FusionConcatFunction.apply(x, sd_flow2, s2_flow2, self.div_flow)
 
 
 class CorrelationCatFunction(Function):
@@ -182,30 +250,34 @@ def flownet2c_forward(net, inputs):
         return net.upsample1(flow2 * net.div_flow)
 
 
+def flownet2_train_forward(net, inputs):
+    """models.FlowNet2.forward (models.py:120-185) with the warp groups fused, differentiable when grad mode is on.
+    net: the reference's FlowNet2; inputs [B,3,2,H,W].  Returns what net.forward returns (flownetfusion's flow).
+    The FlowNetC stage runs through CorrelationCat, concat1 / concat2 through WarpConcat(upsample="bilinear") and
+    concat3 through FusionConcat: neither the x4 upsampled flows nor their gradients are materialised."""
+    div = float(net.div_flow)
+    x = _normalise(inputs, net.rgb_max)
+    x = torch.cat((x[:, :, 0], x[:, :, 1]), dim=1).float()
+    warp_concat = WarpConcat(div, upsample="bilinear")
+    # flownetc -> concat1 = (x | img1 warped | flow / div_flow | |img0 - warped|)                models.py:129-138
+    flow2 = _flownetc_pair(net.flownetc, x[:, 0:3], x[:, 3:])[0]
+    concat1 = warp_concat(x, flow2)
+    # flownets1 -> concat2                                                                        models.py:141-150
+    flow2 = net.flownets_1(concat1)[0]
+    concat2 = warp_concat(x, flow2)
+    del concat1
+    # flownets2 and flownetsd -> concat3 = (img0 | sd flow | s2 flow | their norms | the two diff norms)       :153-179
+    s2_flow2 = net.flownets_2(concat2)[0]
+    del concat2
+    sd_flow2 = net.flownets_d(x)[0]
+    return net.flownetfusion(FusionConcat(div)(x, sd_flow2, s2_flow2))
+
+
 def flownet2_forward(net, inputs):
-    """models.FlowNet2.forward (models.py:120-185) with the warp groups fused.  net: the reference's FlowNet2."""
+    """models.FlowNet2.forward (models.py:120-185) with the warp groups fused, for inference: flownet2_train_forward
+    under torch.no_grad.  net: the reference's FlowNet2."""
     with torch.no_grad():
-        div = float(net.div_flow)
-        x = _normalise(inputs, net.rgb_max)
-        x = torch.cat((x[:, :, 0], x[:, :, 1]), dim=1).float()
-        B, _, H, W = x.shape
-        # flownetc -> concat1 = (x | img1 warped | flow / div_flow | |img0 - warped|)            models.py:129-138
-        flow2 = flownetc_forward(net.flownetc, x)[0]
-        concat1 = F2.warp_concat_forward(x, flow2, upsample="bilinear", flow_mul=div, flow_div=div)
-        # flownets1 -> concat2                                                                    models.py:141-150
-        flow2 = net.flownets_1(concat1)[0]
-        concat2 = F2.warp_concat_forward(x, flow2, upsample="bilinear", flow_mul=div, flow_div=div)
-        del concat1
-        # flownets2 and flownetsd -> concat3 = (img0 | sd flow | s2 flow | their norms | the two diff norms)   :153-174
-        s2_flow2 = net.flownets_2(concat2)[0]
-        del concat2
-        sd_flow2 = net.flownets_d(x)[0]
-        concat3 = torch.empty((B, 11, H, W), dtype=torch.float32, device=x.device)
-        F2.warp_concat_forward(x, sd_flow2, upsample="nearest", flow_mul=1.0 / div, flow_div=1.0, out=concat3, ch_x=0, n_x=3,
-                               ch_warped=-1, ch_flow=3, ch_flow_norm=7, ch_diff_norm=9)
-        F2.warp_concat_forward(x, s2_flow2, upsample="nearest", flow_mul=div, flow_div=1.0, out=concat3, ch_x=-1, n_x=0,
-                               ch_warped=-1, ch_flow=5, ch_flow_norm=8, ch_diff_norm=10)
-        return net.flownetfusion(concat3)
+        return flownet2_train_forward(net, inputs)
 
 
 def fused_forward(net, inputs):
@@ -227,9 +299,8 @@ def train_forward(net, inputs):
     models.py:250-253), else FlowNetC's (flow2,) / FlowNet2C's upsample1(flow2 * div_flow)."""
     name = type(net).__name__
     if name == "FlowNet2":
-        raise TypeError("train_forward: FlowNet2 has no differentiable fused data flow (its warp groups read the x4 "
-                        "upsampled flow, whose backward warp_concat_backward does not include); train it on the drop-in "
-                        "modules")
+        raise TypeError("train_forward: FlowNet2 has no differentiable fused data flow here (train_forward covers "
+                        "FlowNetC and FlowNet2C); use fused.flownet2_train_forward(net, inputs)")
     if name == "FlowNet2C":
         x = _normalise(inputs, net.rgb_max)
         flows = _flownetc_pair(net, x[:, :, 0], x[:, :, 1])

@@ -221,12 +221,30 @@ int fn2b200_warp_concat_forward(const float *x, const int64_t *xstride, int C, c
                                 int H, int W, void *stream);
 
 /*
- * Backward of fn2b200_warp_concat_forward for a full-resolution flow (upsample_mode 0; in a training graph the x4
- * upsample stays a module in front of it), C <= 3.  grad_cat: [B, cat_channels, H, W]; the ch_* layout must be the
- * forward's.  grad_x: [B, 2C, H, W] and grad_flow: [B, 2, H, W], contiguous, fully overwritten.  The composition of
- * the reference modules' own backward passes (torch.cat, the division, ChannelNorm with its 1e-9, the subtraction,
- * Resample2d's K6 scatter and K7 flow gradient) in one kernel plus the transpose of the scatter scratch.
- * workspace: fn2b200_warp_concat_backward_workspace(B, C, H, W) bytes, 16-byte aligned.
+ * Backward of fn2b200_warp_concat_forward, C <= 3, flow taken as the forward takes it (flow / fh / fw / upsample_mode /
+ * flow_mul as there).  grad_cat: [B, cat_channels, H, W]; the ch_* layout must be the forward's.  grad_x: [B, 2C, H, W]
+ * and grad_flow: [B, 2, fh, fw] (the gradient of the quarter-resolution flow for upsample_mode 1 / 2), contiguous, fully
+ * overwritten.  The composition of the reference modules' own backward passes (torch.cat, the division, ChannelNorm
+ * with its 1e-9, the subtraction, Resample2d's K6 scatter and K7 flow gradient, then nn.Upsample's backward times
+ * flow_mul) in one kernel plus the transpose of the scatter scratch (grad_x) and, for upsample_mode 1, a pass that adds
+ * the per-tile partial sums of the upsample's adjoint (grad_flow).  The full-resolution flow gradient is never written
+ * to memory, and grad_flow is bit-identical from run to run (no atomics touch it) and whether or not grad_x is wanted.
+ * Either gradient may be NULL: no grad_x = no scatter (and no scratch fill, no transpose), no grad_flow = no K7; both
+ * NULL is a successful no-op, as is B = 0.
+ * workspace: fn2b200_warp_concat_backward_up_workspace(B, C, H, W, upsample_mode, grad_x != NULL) bytes, 16-byte
+ * aligned (0 bytes, and NULL is fine, for upsample_mode 0 / 2 without grad_x).
+ */
+size_t fn2b200_warp_concat_backward_up_workspace(int B, int C, int H, int W, int upsample_mode, int need_x);
+int fn2b200_warp_concat_backward_up(const float *x, const int64_t *xstride, int C, const float *flow, int fh, int fw,
+                                    int upsample_mode, float flow_mul, const float *grad_cat, int cat_channels, int ch_x,
+                                    int n_x, int ch_warped, int ch_flow, float flow_div, int ch_flow_norm,
+                                    int ch_diff_norm, float *grad_x, float *grad_flow, void *workspace,
+                                    size_t workspace_bytes, int B, int H, int W, void *stream);
+
+/*
+ * fn2b200_warp_concat_backward_up for a full-resolution flow (upsample_mode 0, fh = H, fw = W) with both gradients
+ * required (NULL grad_x / grad_flow is an error here).  workspace: fn2b200_warp_concat_backward_workspace(B, C, H, W)
+ * = fn2b200_warp_concat_backward_up_workspace(B, C, H, W, 0, 1) bytes, 16-byte aligned.
  */
 size_t fn2b200_warp_concat_backward_workspace(int B, int C, int H, int W);
 int fn2b200_warp_concat_backward(const float *x, const int64_t *xstride, int C, const float *flow, const float *grad_cat,
