@@ -357,6 +357,7 @@ bool corr_tiled_supported(const CorrParams &p) {
     if (p.W % 4 != 0) return false;  // TMA global strides must be multiples of 16 bytes
     if (p.oW % 4 != 0) return false;  // gradOutput is a TMA source in backward
     if ((p.md - p.pad) % 4 != 0) return false;  // box x start = tile + (md - pad): must stay 16-B aligned
+    if (p.H > 65535) return false;  // the backward's gridDim.y is H
 #define X(S2_, DR_) if (p.s2 == S2_ && p.dr == DR_) return true;
     FN2_TILED_CONFIGS(X)
 #undef X
@@ -372,24 +373,34 @@ static int make_nchw_map(CUtensorMap *m, const float *base, int B, int C, int H,
     return make_tensor_map_f32(m, base, 4, dims, strides, box);
 }
 
+// gridDim.z carries the sample index and is limited to 65535: larger batches run as several launches of at most
+// kMaxZ samples, each with tensor maps and pointers rebased to its first sample (bases stay 16-byte aligned: W % 4 == 0).
+constexpr int kMaxZ = 65535;
+
 template <int S2, int DR>
 static int launch_fwd(const float *in1, const float *in2, float *out, const CorrParams &p,
                       cudaStream_t st) {
     using Cfg = FwdCfg<S2, DR>;
-    CUtensorMap m1, m2;
-    int rc = make_nchw_map(&m1, in1, p.B, p.C, p.H, p.W, kTW, Cfg::CK);
-    if (rc) return rc;
-    rc = make_nchw_map(&m2, in2, p.B, p.C, p.H, p.W, Cfg::F2W, Cfg::CK);
-    if (rc) return rc;
     auto kern = corr_fwd_tiled_kernel<S2, DR>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM);
     if (e != cudaSuccess) return fail((int)e, "correlation_forward: smem attribute (%s)", cudaGetErrorString(e));
     const int nxt = (p.oW + kTW - 1) / kTW;
     const int ngrp = ((p.oH + S2 - 1) / S2 + Cfg::KR - 1) / Cfg::KR;
-    dim3 grid(Cfg::NSG * nxt, S2 * ngrp, p.B);
-    kern<<<grid, 256, Cfg::SMEM, st>>>(m1, m2, out, p);
-    count_launch();
-    return check_launch("correlation_forward(tiled)");
+    const long in_bstride = (long)p.C * p.H * p.W;
+    for (int b0 = 0; b0 < p.B; b0 += kMaxZ) {
+        CorrParams q = p;
+        q.B = p.B - b0 < kMaxZ ? p.B - b0 : kMaxZ;
+        CUtensorMap m1, m2;
+        int rc = make_nchw_map(&m1, in1 + b0 * in_bstride, q.B, p.C, p.H, p.W, kTW, Cfg::CK);
+        if (rc) return rc;
+        rc = make_nchw_map(&m2, in2 + b0 * in_bstride, q.B, p.C, p.H, p.W, Cfg::F2W, Cfg::CK);
+        if (rc) return rc;
+        dim3 grid(Cfg::NSG * nxt, S2 * ngrp, q.B);
+        kern<<<grid, 256, Cfg::SMEM, st>>>(m1, m2, out + b0 * p.out_bstride, q);
+        count_launch();
+        if ((rc = check_launch("correlation_forward(tiled)"))) return rc;
+    }
+    return 0;
 }
 
 template <int S2, int DR, int WHICH, bool ACT>
@@ -397,23 +408,31 @@ static int launch_bwd(const float *other, const float *gout, float *gin, const C
                       cudaStream_t st) {
     using Cfg = BwdCfg<S2, DR, WHICH, ACT>;
     static_assert(Cfg::SMEM <= 232448, "tiled backward stage ring exceeds the 227 KB of shared memory per block");
-    // gradOutput (and activation) maps: D planes per sample, p.g_bstride elements apart
-    CUtensorMap mo, mg, ma;
-    int rc = make_nchw_map(&mo, other, p.B, p.C, p.H, p.W, Cfg::FW, Cfg::CB);
-    if (rc) return rc;
-    rc = make_nchw_map(&mg, gout, p.B, p.D, p.oH, p.oW, Cfg::GW, Cfg::DS, p.g_bstride);
-    if (rc) return rc;
-    if (ACT && (rc = make_nchw_map(&ma, p.act, p.B, p.D, p.oH, p.oW, Cfg::GW, Cfg::DS, p.g_bstride))) return rc;
-    if (!ACT) ma = mg;                           // not read
     auto kern = corr_bwd_tiled_kernel<S2, DR, WHICH, ACT>;
     cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)Cfg::SMEM);
     if (e != cudaSuccess) return fail((int)e, "correlation_backward: smem attribute (%s)", cudaGetErrorString(e));
     const int nxt = (p.W + kTW - 1) / kTW;
     const int ncb = (p.C + Cfg::CB - 1) / Cfg::CB;
-    dim3 grid(nxt * ncb, p.H, p.B);
-    kern<<<grid, 256, Cfg::SMEM, st>>>(mo, mg, ma, gin, p);
-    count_launch();
-    return check_launch("correlation_backward(tiled)");
+    const long in_bstride = (long)p.C * p.H * p.W;
+    // gridDim.y = H: corr_tiled_supported keeps H <= 65535; gridDim.z = samples, chunked as in launch_fwd
+    for (int b0 = 0; b0 < p.B; b0 += kMaxZ) {
+        CorrParams q = p;
+        q.B = p.B - b0 < kMaxZ ? p.B - b0 : kMaxZ;
+        if (ACT) q.act = p.act + b0 * p.g_bstride;
+        // gradOutput (and activation) maps: D planes per sample, p.g_bstride elements apart
+        CUtensorMap mo, mg, ma;
+        int rc = make_nchw_map(&mo, other + b0 * in_bstride, q.B, p.C, p.H, p.W, Cfg::FW, Cfg::CB);
+        if (rc) return rc;
+        rc = make_nchw_map(&mg, gout + b0 * p.g_bstride, q.B, p.D, p.oH, p.oW, Cfg::GW, Cfg::DS, p.g_bstride);
+        if (rc) return rc;
+        if (ACT && (rc = make_nchw_map(&ma, q.act, q.B, p.D, p.oH, p.oW, Cfg::GW, Cfg::DS, p.g_bstride))) return rc;
+        if (!ACT) ma = mg;                           // not read
+        dim3 grid(nxt * ncb, p.H, q.B);
+        kern<<<grid, 256, Cfg::SMEM, st>>>(mo, mg, ma, gin + b0 * in_bstride, q);
+        count_launch();
+        if ((rc = check_launch("correlation_backward(tiled)"))) return rc;
+    }
+    return 0;
 }
 
 template <int S2, int DR, bool ACT>

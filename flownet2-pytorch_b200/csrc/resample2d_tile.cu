@@ -501,14 +501,22 @@ int resample2d_backward_tile(const float *img, const int64_t *is, const float *f
         case 3: FN2_B(3, PY, SC); break;                                                                               \
         default: FN2_B(0, PY, SC); break;                                                                              \
     }
+// scatter 2 has C <= 3 (see above): no runtime-C instantiation
+#define FN2_BC2(PY)                                                                                                      \
+    switch (C) {                                                                                                       \
+        case 1: FN2_B(1, PY, 2); break;                                                                                \
+        case 2: FN2_B(2, PY, 2); break;                                                                                \
+        default: FN2_B(3, PY, 2); break;                                                                               \
+    }
 #define FN2_BS(PY)                                                                                                       \
     switch (scatter) {                                                                                                 \
         case 0: FN2_BC(PY, 0) break;                                                                                   \
         case 1: FN2_BC(PY, 1) break;                                                                                   \
-        default: FN2_BC(PY, 2) break;                                                                                  \
+        default: FN2_BC2(PY) break;                                                                                    \
     }
     if (PYc == 4) { FN2_BS(4) } else if (PYc == 2) { FN2_BS(2) } else { FN2_BS(1) }
 #undef FN2_BS
+#undef FN2_BC2
 #undef FN2_BC
 #undef FN2_B
     count_launch();
