@@ -287,7 +287,7 @@ corr_fwd_tc_kernel(const __grid_constant__ CUtensorMap m1h, const __grid_constan
 //
 //   gI1[c, p] = 1/C sum_q G1[p, q] f2[c, q],   G1[p, q] = gO[(q - p), p]          (|q - p| <= 10)
 //   gI2[c, q] = 1/C sum_p G2[q, p] f1[c, p],   G2[q, p] = gO[(q - p), p]
-// per parity class: D[128 tile px][C] += A[128][144] * B[144 halo px][C] over the 7 halo-row units, accumulated in
+// per parity class: D[128 tile px][C] += A[128][144] * B[144 halo px][C] over the halo-row units, accumulated in
 // registers (warpgroup wg: tile pixels [64 wg, 64 wg + 64), an m64 x nC fragment) for the whole tile.
 //   A = the banded gradOutput matrix, built per unit by the warpgroup's own threads straight from the fp32 gradOutput
 //       planes (bf16 hi/lo split on the fly) into an MN-major SW128 layout [k][64 pixels] (two buffers per warpgroup,
@@ -331,6 +331,17 @@ template <> __device__ __forceinline__ void wgmma_bwd<1>(float (&d)[32], uint64_
 template <> __device__ __forceinline__ void wgmma_bwd<2>(float (&d)[64], uint64_t da, uint64_t db) { wgmma_m64n128k16_mn(d, da, db); }
 template <> __device__ __forceinline__ void wgmma_bwd<3>(float (&d)[96], uint64_t da, uint64_t db) { wgmma_m64n192k16_mn(d, da, db); }
 template <> __device__ __forceinline__ void wgmma_bwd<4>(float (&d)[128], uint64_t da, uint64_t db) { wgmma_m64n256k16_mn(d, da, db); }
+
+// Ring slots [b, b + n) that the calling warpgroup does not read: wait for each fill, then release it.  Releasing a
+// slot before its fill has landed would complete the previous phase, and a slot refilled before this warpgroup saw its
+// current phase would make the parity of its next wait on the slot ambiguous.
+__device__ __forceinline__ void tc_skip_slots(uint64_t *full, uint64_t *empty, uint32_t b, int n, int bst) {
+    for (int i = 0; i < n; ++i, ++b) {
+        const int s = b % bst;
+        mbar_wait(&full[s], (b / bst) & 1);
+        mbar_arrive(&empty[s]);
+    }
+}
 
 // Both gradients in ONE launch: global tiles [t_begin, t_end) of [0, 2 ntiles).  One gradient only: tile g < ntiles
 // is tile g of gradInput1 (B = input2's halo, maps m2h / m2l), tile g >= ntiles is tile g - ntiles of gradInput2
@@ -458,7 +469,10 @@ corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constan
         for (int i = 0; i < C / 2; ++i) acc[i] = 0.f;
         wgmma_fence_operands(acc);
         int prev = -1;                                         // ring slot read by the wgmma group in flight
-        for (int u = 0; u < TC_NU; ++u, ++ucount) {
+        // warpgroup wg's pixel rows 4 wg .. 4 wg + 3 only meet units wg .. wg + 5: the other unit's A would be all zero.
+        // Warpgroup 1 releases unit 0's slots once it has built the A of unit 1, warpgroup 0 unit 6's after its epilogue.
+        if (wg == 1) bcount += 2 * TB_NG;
+        for (int u = wg; u < TC_NU - 1 + wg; ++u, ++ucount) {
             // buffer ucount & 1 was last read by unit ucount - 2, complete since unit ucount - 1's first wait
             unsigned char *ah = aw + (ucount & 1) * TB_ASTG, *al = ah + TB_AHL;
 #pragma unroll
@@ -498,6 +512,7 @@ corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constan
             }
             fence_proxy_async();                               // generic-proxy writes -> visible to the tensor core
             named_barrier_sync(1 + wg, 128);                   // the warpgroup's whole A is written
+            if (u == 1 && wg == 1) tc_skip_slots(b_full, b_empty, bcount - 2 * TB_NG, 2 * TB_NG, bst);
             const uint32_t ah32 = smem_u32(ah), al32 = smem_u32(al);
             for (int gr = 0; gr < TB_NG; ++gr)
 #pragma unroll
@@ -532,6 +547,10 @@ corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constan
             for (int j = 0; j < 4; ++j)
                 if ((j >> 1) ? ok1 : ok0)
                     __stcs(o + 16 * (j >> 1) + (long)(8 * i + 2 * q + (j & 1)) * plane, acc[4 * i + j] * inv_nelems);
+        if (wg == 0) {
+            tc_skip_slots(b_full, b_empty, bcount, 2 * TB_NG, bst);
+            bcount += 2 * TB_NG;
+        }
     }
 }
 
