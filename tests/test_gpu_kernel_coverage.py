@@ -21,6 +21,7 @@ from torch.profiler import ProfilerActivity, profile
 
 import torch_ref
 import upsample_ref as ur
+from guarded import SENTINEL, Arena
 from kernel_manifest import KERNELS
 from oracle import cpu as orc
 from util import assert_close
@@ -28,10 +29,6 @@ from util import assert_close
 pytestmark = pytest.mark.gpu
 P = ctypes.c_void_p
 TOL = 1e-4
-POISON32 = 0x7FC0DEAD           # a quiet NaN as fp32
-POISON16 = 0x7FC07FC0           # two quiet NaNs as fp16 and as bf16
-LEAD, TAIL = 256, 256           # guard bytes in front of / behind every view
-SENTINEL = 12345.0              # finite value of elements a call must leave alone
 
 
 def _f2():
@@ -45,48 +42,6 @@ def _stream():
 
 def _p(t):
     return P(t.data_ptr()) if t is not None else P(0)
-
-
-class Arena(object):
-    """Views carved out of poisoned allocations, and the check that nothing outside them changed."""
-
-    def __init__(self):
-        self.items = []
-
-    def _alloc(self, nbytes, misalign, poison):
-        words = (LEAD + misalign + nbytes + TAIL + 3) // 4
-        raw = torch.full((words,), poison, dtype=torch.int32, device="cuda")
-        return raw, LEAD + misalign
-
-    def out(self, shape, dtype=torch.float32, misalign=0, fill=None):
-        """An output view: poisoned (or `fill`ed), guarded; must come back finite."""
-        es = torch.empty((), dtype=dtype).element_size()
-        n = int(np.prod(shape))
-        raw, start = self._alloc(n * es, misalign, POISON32 if es == 4 else POISON16)
-        v = raw.view(torch.uint8)[start:start + n * es].view(dtype).view(shape)
-        if fill is not None:
-            v.fill_(fill)
-        self.items.append((raw, raw.clone(), start, n * es, v, "output %s" % (tuple(shape),)))
-        return v
-
-    def workspace(self, nbytes):
-        """A workspace of exactly nbytes (None for 0); its contents are scratch, only its guards are checked."""
-        if not nbytes:
-            return None
-        raw, start = self._alloc(nbytes, 0, POISON32)
-        v = raw.view(torch.uint8)[start:start + nbytes]
-        self.items.append((raw, raw.clone(), start, nbytes, None, "workspace of %d bytes" % nbytes))
-        return v
-
-    def check(self):
-        torch.cuda.synchronize()
-        for raw, orig, start, nbytes, view, what in self.items:
-            b, o = raw.view(torch.uint8), orig.view(torch.uint8)
-            assert torch.equal(b[:start], o[:start]), "%s: the guard in front was written" % what
-            assert torch.equal(b[start + nbytes:], o[start + nbytes:]), "%s: the guard behind was written" % what
-            if view is not None:
-                assert bool(torch.isfinite(view).all()), "%s: %d elements not finite (never written?)" % (
-                    what, int((~torch.isfinite(view)).sum()))
 
 
 def _kernel_names(prof):
