@@ -18,8 +18,9 @@
 //                    [144 rows x 128 B] = one 18-KB box, 128-byte swizzle; halo outside the image = TMA
 //                    out-of-bounds zero fill = the layer's zero padding
 //   warps 0-7      : two warpgroups, one per 64 tile pixels: wgmma m64n144k16 (hi slot: hi*hi and lo*hi, lo slot:
-//                    hi*lo, 4 k-steps each) into an fp32 register accumulator, then each thread stores the band entries
-//                    of its fragment, scaled by 1/C, to out[n][(tj,ti)][y][x]
+//                    hi*lo, 4 k-steps each) into an fp32 register accumulator; each warp then moves the band entries
+//                    of its fragment, scaled by 1/C, through a private shared-memory buffer to out[n][(tj,ti)][y][x],
+//                    16 pixels x 2 displacement planes per store instruction
 #include "wgmma.cuh"
 #include <cuda_bf16.h>
 #include <stdlib.h>
@@ -40,9 +41,16 @@ constexpr int TC_ABLK = 128 * 128;             // bytes of one A k-block (128 ro
 constexpr int TC_BBLK = TC_N * 128;            // bytes of one B k-block (144 rows x 128 B)
 constexpr int TC_NBAR = 2 * TC_MAXKB + 2 * TC_MAXBST;
 constexpr int TC_SMEM_MAX = 232448;            // 227 KB opt-in limit per CTA (sm_90)
-// A_hi and A_lo blocks, then bst ring slots of one 18-KB box each (+ 1 KB for the 1024-byte alignment of the swizzle atoms)
+// Forward epilogue staging: each consumer warp transposes its band through a private buffer [ti][px] of its 16 tile
+// pixels, one displacement row ti every TC_SPITCH floats.  The pitch makes the fill conflict-free: for one
+// accumulator register, lane (pxa, q) writes float (2q - pxa + k) * 20 + pxa, and 8q + 13 pxa is distinct mod 32 for
+// all 32 lanes (pitch 16 would put the 4 lanes of a pixel in one bank).
+constexpr int TC_SPITCH = 20;
+constexpr int TC_SBUF = (TC_DS - 1) * TC_SPITCH + TC_TW;     // floats per warp
+// A_hi and A_lo blocks, then bst ring slots of one 18-KB box each, the mbarriers, the 8 staging buffers (+ 1 KB for
+// the 1024-byte alignment of the swizzle atoms)
 __host__ __device__ constexpr int tc_smem_bytes(int nkb, int bst) {
-    return 2 * nkb * TC_ABLK + bst * TC_BBLK + TC_NBAR * 8 + 1024;
+    return 2 * nkb * TC_ABLK + bst * TC_BBLK + TC_NBAR * 8 + 8 * TC_SBUF * 4 + 1024;
 }
 
 // ------------------------------------------------------------------------------------------------
@@ -167,6 +175,7 @@ corr_fwd_tc_kernel(const __grid_constant__ CUtensorMap m1h, const __grid_constan
     uint64_t *bars = reinterpret_cast<uint64_t *>(sB + bst * TC_BBLK);
     uint64_t *a_full = bars, *a_empty = bars + TC_MAXKB;
     uint64_t *b_full = bars + 2 * TC_MAXKB, *b_empty = b_full + TC_MAXBST;
+    float *stage = reinterpret_cast<float *>(bars + TC_NBAR);  // [consumer warp][TC_SBUF]
 
     if (tid == 0) {
         prefetch_tensormap(&m1h); prefetch_tensormap(&m1l);
@@ -212,6 +221,9 @@ corr_fwd_tc_kernel(const __grid_constant__ CUtensorMap m1h, const __grid_constan
         const int wg = warp >> 2, wq = warp & 3;
         // accumulator fragment: rows 16 wq + lane / 4 (+ 8) of the warpgroup = tile row 4 wg + wq, columns pxa (+ 8)
         const int py_t = 4 * wg + wq, pxa = lane >> 2, q = lane & 3;
+        // store role: tile pixel sx of the fragment row, displacement column ti = t + sd of a store pair
+        const int sx = lane & 15, sd = lane >> 4;
+        float *sbuf = stage + warp * TC_SBUF;
         // 1/(k*k*C): exact for power-of-two C (FlowNetC: 256) -> bit-identical to the reference's divide; otherwise
         // within 1 ulp.
         const float inv_nelems = 1.0f / (float)C;
@@ -223,8 +235,8 @@ corr_fwd_tc_kernel(const __grid_constant__ CUtensorMap m1h, const __grid_constan
         for (int tn = blockIdx.x, w = w0; tc_next_seg(tn, w, full, w1, sg); ++it) {
             const int ua = sg.ua, ub = sg.ub;
             const TcTile T = tc_decode(sg.t, nxt, nyt);
-            const int yc = T.yc0 + py_t, xc = T.xc0 + pxa;
-            const bool ok0 = (yc < Hc) && (xc < Wc), ok1 = (yc < Hc) && (xc + 8 < Wc);
+            const int yc = T.yc0 + py_t, xc = T.xc0 + sx;
+            const bool ok = (yc < Hc) && (xc < Wc);
             float *ob = out + (long)T.n * out_bstride + (long)(2 * yc + T.py) * W + (2 * xc + T.px);
             for (int u = ua; u < ub; ++u) {
                 float acc[TC_N / 2];
@@ -262,21 +274,36 @@ corr_fwd_tc_kernel(const __grid_constant__ CUtensorMap m1h, const __grid_constan
                 mbar_arrive(&b_empty[prev]);
                 if (prev_a >= 0) mbar_arrive(&a_empty[prev_a]);
                 // accumulator column c = hrl * 36 + qx (halo row hrl of the unit, halo column qx) of tile pixel
-                // (py_t, px) is displacement (tj, ti) = (u * 4 + hrl - py_t, qx - px) - (10, 10), if inside the band
+                // (py_t, px) is displacement (tj, ti) = (u * 4 + hrl - py_t, qx - px) - (10, 10), if inside the band.
+                // Per halo row, tj is the same for the whole warp (its fragment rows are one tile row), and each of
+                // its 16 pixels has exactly 21 in-band columns among the row's 36, so the warp's buffer [ti][px] is
+                // wholly rewritten by each pass.  Storing from the buffer writes 16 consecutive pixels of 2
+                // displacement planes per instruction (2 lines), where storing from the fragment wrote one value
+                // per lane to up to 32 different planes.
                 const int tjb = u * TC_UR - py_t;
 #pragma unroll
-                for (int i = 0; i < TC_N / 8; ++i)
+                for (int hrl = 0; hrl < TC_UR; ++hrl) {
+                    const int tj = tjb + hrl;
+                    if ((unsigned)tj >= (unsigned)TC_DS) continue;     // warp-uniform
 #pragma unroll
-                    for (int j = 0; j < 4; ++j) {
-                        const int c = 8 * i + 2 * q + (j & 1);
-                        const int hrl = c / TC_HW;
-                        const int ti = c - hrl * TC_HW - pxa - 8 * (j >> 1), tj = tjb + hrl;
-                        if (((j >> 1) ? ok1 : ok0) && (unsigned)ti < (unsigned)TC_DS && (unsigned)tj < (unsigned)TC_DS) {
-                            float v = acc[4 * i + j] * inv_nelems;
-                            if (act) v = v > 0.f ? v : v * leaky;      // fused nn.LeakyReLU (FlowNetC.py:87), warp-uniform
-                            __stcs(ob + 16 * (j >> 1) + (long)(tj * TC_DS + ti) * plane, v);
+                    for (int i = TC_HW * hrl / 8; i <= (TC_HW * hrl + TC_HW - 1) / 8; ++i)
+#pragma unroll
+                        for (int j = 0; j < 4; ++j) {
+                            const int x = pxa + 8 * (j >> 1);
+                            const int ti = 8 * i + 2 * q + (j & 1) - TC_HW * hrl - x;
+                            if ((unsigned)ti < (unsigned)TC_DS) {           // implies the column lies in halo row hrl
+                                float v = acc[4 * i + j] * inv_nelems;
+                                if (act) v = v > 0.f ? v : v * leaky;      // fused nn.LeakyReLU (FlowNetC.py:87), warp-uniform
+                                sbuf[ti * TC_SPITCH + x] = v;
+                            }
                         }
-                    }
+                    __syncwarp();
+                    float *o = ob + (long)(tj * TC_DS + sd) * plane;
+#pragma unroll
+                    for (int t = 0; t < TC_DS; t += 2)
+                        if (ok && t + sd < TC_DS) __stcs(o + (long)t * plane, sbuf[(t + sd) * TC_SPITCH + sx]);
+                    __syncwarp();                                   // read before the next pass overwrites
+                }
             }
         }
     }
