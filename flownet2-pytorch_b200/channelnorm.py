@@ -3,32 +3,24 @@
 ``norm_deg`` is stored and passed through but, as in the reference kernels, always L2.
 """
 import torch
-from torch.autograd import Function
-from torch.autograd.function import once_differentiable
 from torch.nn.modules.module import Module
 
 from . import functional as F2
+from .ops import fn2b200
 
 
-class ChannelNormFunction(Function):
+def channelnorm(input1, norm_deg=2):
+    """torch.ops.fn2b200.channelnorm_forward (differentiable; fp16 / bf16 run natively, other dtypes through fp32 and
+    back)."""
+    F2._require_cuda(input1)
+    out = fn2b200.channelnorm_forward(input1, norm_deg)
+    return out if out.dtype == input1.dtype else out.to(input1.dtype)
 
-    @staticmethod
-    def forward(ctx, input1, norm_deg=2):
-        out = F2.channelnorm_forward(input1, norm_deg)
-        if input1.dtype != torch.float32:
-            out = out.to(input1.dtype)
-        ctx.save_for_backward(input1, out)
-        ctx.norm_deg = norm_deg
-        return out
 
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, grad_output):
-        input1, output = ctx.saved_tensors
-        g = F2.channelnorm_backward(input1, output, grad_output, ctx.norm_deg)
-        if g.dtype != input1.dtype:
-            g = g.to(input1.dtype)
-        return g, None
+class ChannelNormFunction(object):
+    """reference: channelnorm.py:5-28 -- ``ChannelNormFunction.apply(input1, norm_deg)``, forwarded to the operator
+    (``channelnorm``)."""
+    apply = forward = staticmethod(channelnorm)
 
 
 class ChannelNorm(Module):
@@ -38,7 +30,7 @@ class ChannelNorm(Module):
         self.norm_deg = norm_deg
 
     def forward(self, input1):
-        return ChannelNormFunction.apply(input1, self.norm_deg)
+        return channelnorm(input1, self.norm_deg)
 
     def extra_repr(self):
         return "norm_deg=%d" % self.norm_deg

@@ -34,154 +34,96 @@ and hyper-parameters are used as they are) and run the same data flow with the g
 * ``FusionConcat`` / ``FusionConcatFunction`` -- the 11-channel concat3 of the fusion stage from x and the
   quarter-resolution FlowNetSD / FlowNetS2 flows, same scheme (nearest upsample).
 
+Each of these ops is one ``torch.ops.fn2b200`` operator with a fake kernel and an autograd formula (``ops``): the
+training and inference forwards trace under torch.compile without a graph break and capture into CUDA graphs.
+
 Results agree with the unfused graph to rounding (tests/test_gpu_parity.py::test_fused_forwards_match_unfused_models,
 tests/test_gpu_corr_cat.py).
 """
 import torch
-from torch.autograd import Function
-from torch.autograd.function import once_differentiable
 
 from . import functional as F2
+from .ops import fn2b200
 
 
-def _pad_channels(gx, channels):
-    """gx [B, 2C, H, W] -> [B, channels, H, W]: odd trailing channels of x take no part in the op."""
-    if channels > gx.size(1):
-        gx = torch.cat((gx, gx.new_zeros(gx.size(0), channels - gx.size(1), gx.size(2), gx.size(3))), 1)
-    return gx
+def warp_concat(x, flow, div_flow=20.0, upsample=None):
+    """torch.ops.fn2b200.warp_concat_forward with models.py:138's concat1 layout (differentiable): x [B, 2C, H, W] ->
+    cat(x, Resample2d()(x[:, C:], flow_up), flow_up / div_flow, ChannelNorm()(x[:, :C] - warped)), 3C + 3 channels."""
+    F2._require_cuda(x, flow)
+    C = x.size(1) // 2
+    div = float(div_flow)
+    return fn2b200.warp_concat_forward(x, flow, C, F2.UPSAMPLE_MODES[upsample], div, div, 3 * C + 3, 0, 2 * C, 2 * C, 3 * C,
+                                       -1, 3 * C + 2)
 
 
-class WarpConcatFunction(Function):
+class WarpConcatFunction(object):
     """concat1 = cat(x, Resample2d()(x[:, 3:], flow_up), flow_up / div_flow, ChannelNorm()(x[:, :3] - warped)) as one
     differentiable op (models.py:133-138, :145-150).  upsample=None: flow is the full-resolution flow_up.
     upsample="bilinear" / "nearest": flow is the quarter-resolution flow2 and flow_up = nn.Upsample(scale_factor=4,
     mode=upsample)(flow2 * div_flow) (models.py:130, :142) -- folded into the kernels, so the full-resolution flow and
     its gradient are never materialised.  forward is one kernel; backward one kernel plus the passes that finish the
-    gradients asked for (only those in ctx.needs_input_grad are computed)."""
-
-    @staticmethod
-    def forward(ctx, x, flow, div_flow=20.0, upsample=None):
-        ctx.save_for_backward(x, flow)
-        ctx.div_flow, ctx.upsample = float(div_flow), upsample
-        return F2.warp_concat_forward(x, flow, C=x.size(1) // 2, upsample=upsample, flow_mul=ctx.div_flow,
-                                      flow_div=ctx.div_flow)
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, grad_cat):
-        x, flow = ctx.saved_tensors
-        need_x, need_flow = ctx.needs_input_grad[:2]
-        gx, gf = F2.warp_concat_backward(x, flow, grad_cat, C=x.size(1) // 2, flow_div=ctx.div_flow, upsample=ctx.upsample,
-                                         flow_mul=ctx.div_flow, need_x=need_x, need_flow=need_flow)
-        return (_pad_channels(gx, x.size(1)) if need_x else None), gf, None, None
+    gradients asked for (only those in ctx.needs_input_grad are computed).  ``apply(x, flow, div_flow, upsample)`` is
+    ``warp_concat``."""
+    apply = staticmethod(warp_concat)
 
 
 class WarpConcat(torch.nn.Module):
-    """nn.Module form of WarpConcatFunction: WarpConcat(div_flow, upsample)(x, flow) -> the (3C + 3)-channel concat."""
+    """nn.Module form of warp_concat: WarpConcat(div_flow, upsample)(x, flow) -> the (3C + 3)-channel concat."""
 
     def __init__(self, div_flow=20.0, upsample=None):
         super(WarpConcat, self).__init__()
         self.div_flow, self.upsample = div_flow, upsample
 
     def forward(self, x, flow):
-        return WarpConcatFunction.apply(x, flow, self.div_flow, self.upsample)
+        return warp_concat(x, flow, self.div_flow, self.upsample)
 
 
-# concat3 of models.py:179: (img0 | sd flow | s2 flow | |sd flow| | |s2 flow| | sd diff norm | s2 diff norm), each flow
-# the nearest x4 upsample of its quarter-resolution flow2 (sd: / div_flow, models.py:167; s2: * div_flow, :154)
-_FUSION_SD = dict(ch_x=0, n_x=3, ch_warped=-1, ch_flow=3, ch_flow_norm=7, ch_diff_norm=9)
-_FUSION_S2 = dict(ch_x=-1, n_x=0, ch_warped=-1, ch_flow=5, ch_flow_norm=8, ch_diff_norm=10)
+def fusion_concat(x, sd_flow2, s2_flow2, div_flow=20.0):
+    """torch.ops.fn2b200.fusion_concat (differentiable): concat3 of models.py:153-179, (x [B,6,H,W], sd_flow2, s2_flow2
+    [B,2,H/4,W/4]) -> [B,11,H,W] = (img0 | sd flow | s2 flow | their norms | the two diff norms), each flow the nearest
+    x4 upsample of its quarter-resolution flow2.  forward = two warp-concat kernels into one buffer; backward = two
+    warp-concat backward passes, each reading its own channels of the concat gradient, the x gradients summed."""
+    F2._require_cuda(x, sd_flow2, s2_flow2)
+    return fn2b200.fusion_concat(x, sd_flow2, s2_flow2, float(div_flow))
 
 
-class FusionConcatFunction(Function):
-    """concat3 of models.py:153-179 as one differentiable op: (x [B,6,H,W], sd_flow2, s2_flow2 [B,2,H/4,W/4]) ->
-    [B,11,H,W].  forward = two warp_concat_forward calls into one buffer; backward = two warp_concat_backward calls,
-    each reading its own channels of the concat gradient, the x gradients summed."""
-
-    @staticmethod
-    def forward(ctx, x, sd_flow2, s2_flow2, div_flow=20.0):
-        ctx.save_for_backward(x, sd_flow2, s2_flow2)
-        ctx.div_flow = div = float(div_flow)
-        B, _, H, W = x.shape
-        concat3 = torch.empty((B, 11, H, W), dtype=torch.float32, device=x.device)
-        F2.warp_concat_forward(x, sd_flow2, upsample="nearest", flow_mul=1.0 / div, flow_div=1.0, out=concat3, **_FUSION_SD)
-        F2.warp_concat_forward(x, s2_flow2, upsample="nearest", flow_mul=div, flow_div=1.0, out=concat3, **_FUSION_S2)
-        return concat3
-
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, grad_cat):
-        x, sd_flow2, s2_flow2 = ctx.saved_tensors
-        need_x, need_sd, need_s2 = ctx.needs_input_grad[:3]
-        div = ctx.div_flow
-        gx = g_sd = g_s2 = None
-        if need_x or need_sd:
-            gx, g_sd = F2.warp_concat_backward(x, sd_flow2, grad_cat, flow_div=1.0, upsample="nearest", flow_mul=1.0 / div,
-                                               need_x=need_x, need_flow=need_sd, **_FUSION_SD)
-        if need_x or need_s2:
-            gx2, g_s2 = F2.warp_concat_backward(x, s2_flow2, grad_cat, flow_div=1.0, upsample="nearest", flow_mul=div,
-                                                need_x=need_x, need_flow=need_s2, **_FUSION_S2)
-            gx = gx2 if gx is None else gx.add_(gx2)
-        return (_pad_channels(gx, x.size(1)) if need_x else None), g_sd, g_s2, None
+class FusionConcatFunction(object):
+    """concat3 of models.py:153-179 as one differentiable op: ``apply(x, sd_flow2, s2_flow2, div_flow)`` is
+    ``fusion_concat``."""
+    apply = staticmethod(fusion_concat)
 
 
 class FusionConcat(torch.nn.Module):
-    """nn.Module form of FusionConcatFunction: FusionConcat(div_flow)(x, sd_flow2, s2_flow2) -> the 11-channel concat3."""
+    """nn.Module form of fusion_concat: FusionConcat(div_flow)(x, sd_flow2, s2_flow2) -> the 11-channel concat3."""
 
     def __init__(self, div_flow=20.0):
         super(FusionConcat, self).__init__()
         self.div_flow = div_flow
 
     def forward(self, x, sd_flow2, s2_flow2):
-        return FusionConcatFunction.apply(x, sd_flow2, s2_flow2, self.div_flow)
+        return fusion_concat(x, sd_flow2, s2_flow2, self.div_flow)
 
 
-class CorrelationCatFunction(Function):
-    """torch.cat((redir, LeakyReLU(leaky_slope)(Correlation(...)(input1, input2))), 1) -> fp32 [B, R + D, oH, oW]
-    (FlowNetC.py:86-92 from `out_corr = self.corr(...)` to `in_conv3_1`)."""
+def correlation_cat(redir, input1, input2, pad_size, kernel_size, max_displacement, stride1, stride2, corr_multiply=1,
+                    leaky_slope=0.1):
+    """torch.ops.fn2b200.correlation_forward_cat (differentiable): torch.cat((redir, LeakyReLU(leaky_slope)(
+    Correlation(...)(input1, input2))), 1) -> fp32 [B, R + D, oH, oW] (FlowNetC.py:86-92 from `out_corr = self.corr(...)`
+    to `in_conv3_1`).  The backward is one correlation_backward_cat launch on the tensor-core path: it reads the
+    correlation's gradient straight out of the concat gradient and LeakyReLU's derivative from the saved concat."""
+    F2._require_cuda(redir, input1, input2)
+    return fn2b200.correlation_forward_cat(redir, input1, input2, pad_size, kernel_size, max_displacement, stride1,
+                                           stride2, corr_multiply, float(leaky_slope))[0]
 
-    @staticmethod
-    def forward(ctx, redir, input1, input2, pad_size, kernel_size, max_displacement, stride1, stride2, corr_multiply=1,
-                leaky_slope=0.1):
-        B, C, H, W = input1.shape
-        D, oH, oW = F2.correlation_out_shape(C, H, W, pad_size, kernel_size, max_displacement, stride1, stride2)
-        R = redir.size(1)
-        if redir.dim() != 4 or (redir.size(0), redir.size(2), redir.size(3)) != (B, oH, oW):
-            raise ValueError("CorrelationCat: redir %s does not match the correlation output [%d, D, %d, %d]"
-                             % (tuple(redir.shape), B, oH, oW))
-        cat = torch.empty((B, R + D, oH, oW), dtype=torch.float32, device=input1.device)
-        cat[:, :R].copy_(redir)
-        cat, ws = F2.correlation_forward_cat(input1, input2, cat, R, leaky_slope, pad_size, kernel_size, max_displacement,
-                                             stride1, stride2, corr_multiply, return_workspace=True)
-        ctx.prm = (pad_size, kernel_size, max_displacement, stride1, stride2, corr_multiply)
-        ctx.leaky_slope, ctx.nredir, ctx.redir_dtype = float(leaky_slope), R, redir.dtype
-        # the bf16 hi/lo copies of the inputs, for a single-launch backward; dropped with ctx (see CorrelationFunction)
-        ctx.workspace = ws if (ctx.needs_input_grad[1] or ctx.needs_input_grad[2]) else None
-        ctx.save_for_backward(input1, input2, cat)
-        return cat
 
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, grad_cat):
-        input1, input2, cat = ctx.saved_tensors
-        need_r, need1, need2 = ctx.needs_input_grad[:3]
-        gr = grad_cat[:, :ctx.nredir].to(ctx.redir_dtype) if need_r else None
-        g1 = g2 = None
-        if need1 or need2:
-            pad_size, kernel_size, max_displacement, stride1, stride2, corr_multiply = ctx.prm
-            g1, g2 = F2.correlation_backward_cat(input1, input2, grad_cat, cat, ctx.nredir, ctx.leaky_slope, pad_size,
-                                                 kernel_size, max_displacement, stride1, stride2, corr_multiply,
-                                                 need1=need1, need2=need2, workspace=ctx.workspace)
-        ctx.workspace = None
-        if g1 is not None and g1.dtype != input1.dtype:
-            g1 = g1.to(input1.dtype)
-        if g2 is not None and g2.dtype != input2.dtype:
-            g2 = g2.to(input2.dtype)
-        return (gr, g1, g2) + (None,) * 7
+class CorrelationCatFunction(object):
+    """torch.cat((redir, LeakyReLU(leaky_slope)(Correlation(...)(input1, input2))), 1) as one differentiable op:
+    ``apply(redir, input1, input2, pad_size, kernel_size, max_displacement, stride1, stride2, corr_multiply,
+    leaky_slope)`` is ``correlation_cat``."""
+    apply = staticmethod(correlation_cat)
 
 
 class CorrelationCat(torch.nn.Module):
-    """nn.Module form of CorrelationCatFunction: CorrelationCat(pad_size, kernel_size, max_displacement, stride1, stride2,
+    """nn.Module form of correlation_cat: CorrelationCat(pad_size, kernel_size, max_displacement, stride1, stride2,
     corr_multiply, leaky_slope)(redir, input1, input2) -> the fp32 concat `redir | LeakyReLU(corr(input1, input2))`."""
 
     def __init__(self, pad_size, kernel_size, max_displacement, stride1, stride2, corr_multiply=1, leaky_slope=0.1):
@@ -190,8 +132,8 @@ class CorrelationCat(torch.nn.Module):
         self.stride1, self.stride2, self.corr_multiply, self.leaky_slope = stride1, stride2, corr_multiply, leaky_slope
 
     def forward(self, redir, input1, input2):
-        return CorrelationCatFunction.apply(redir, input1, input2, self.pad_size, self.kernel_size, self.max_displacement,
-                                            self.stride1, self.stride2, self.corr_multiply, self.leaky_slope)
+        return correlation_cat(redir, input1, input2, self.pad_size, self.kernel_size, self.max_displacement, self.stride1,
+                               self.stride2, self.corr_multiply, self.leaky_slope)
 
 
 def _corr_module(net_c):
@@ -218,9 +160,9 @@ def _flownetc_pair(net_c, x1, x2):
     out_conv3b = net_c.conv3(net_c.conv2(net_c.conv1(x2)))
     out_conv_redir = net_c.conv_redir(out_conv3a)
     corr = _corr_module(net_c)
-    in_conv3_1 = CorrelationCat(corr.pad_size, corr.kernel_size, corr.max_displacement, corr.stride1, corr.stride2,
-                                corr.corr_multiply, net_c.corr_activation.negative_slope)(out_conv_redir, out_conv3a,
-                                                                                          out_conv3b)
+    in_conv3_1 = correlation_cat(out_conv_redir, out_conv3a, out_conv3b, corr.pad_size, corr.kernel_size,
+                                 corr.max_displacement, corr.stride1, corr.stride2, corr.corr_multiply,
+                                 net_c.corr_activation.negative_slope)
     out_conv3_1 = net_c.conv3_1(in_conv3_1.to(out_conv_redir.dtype))
     out_conv4 = net_c.conv4_1(net_c.conv4(out_conv3_1))
     out_conv5 = net_c.conv5_1(net_c.conv5(out_conv4))
@@ -258,19 +200,18 @@ def flownet2_train_forward(net, inputs):
     div = float(net.div_flow)
     x = _normalise(inputs, net.rgb_max)
     x = torch.cat((x[:, :, 0], x[:, :, 1]), dim=1).float()
-    warp_concat = WarpConcat(div, upsample="bilinear")
     # flownetc -> concat1 = (x | img1 warped | flow / div_flow | |img0 - warped|)                models.py:129-138
     flow2 = _flownetc_pair(net.flownetc, x[:, 0:3], x[:, 3:])[0]
-    concat1 = warp_concat(x, flow2)
+    concat1 = warp_concat(x, flow2, div, upsample="bilinear")
     # flownets1 -> concat2                                                                        models.py:141-150
     flow2 = net.flownets_1(concat1)[0]
-    concat2 = warp_concat(x, flow2)
+    concat2 = warp_concat(x, flow2, div, upsample="bilinear")
     del concat1
     # flownets2 and flownetsd -> concat3 = (img0 | sd flow | s2 flow | their norms | the two diff norms)       :153-179
     s2_flow2 = net.flownets_2(concat2)[0]
     del concat2
     sd_flow2 = net.flownets_d(x)[0]
-    return net.flownetfusion(FusionConcat(div)(x, sd_flow2, s2_flow2))
+    return net.flownetfusion(fusion_concat(x, sd_flow2, s2_flow2, div))
 
 
 def flownet2_forward(net, inputs):

@@ -1,6 +1,7 @@
 """Build the three pybind extension modules the reference imports by name -- ``correlation_cuda``,
-``resample2d_cuda``, ``channelnorm_cuda`` (correlation.py:4, resample2d.py:3, channelnorm.py:3) -- as thin ATen glue
-over libfn2b200.so's C ABI (g++ only: no device code lives here).
+``resample2d_cuda``, ``channelnorm_cuda`` (correlation.py:4, resample2d.py:3, channelnorm.py:3) -- and the operator
+library ``fn2b200_ops`` (torch.ops.fn2b200.*, loaded by flownet2_b200.ops) as thin ATen glue over libfn2b200.so's C ABI
+(g++ only: no device code lives here).
 
     python flownet2-pytorch_b200/pybind/build_pybind.py [--force]
 
@@ -17,7 +18,7 @@ from concurrent.futures import ThreadPoolExecutor
 HERE = os.path.dirname(os.path.abspath(__file__))
 PKG = os.path.dirname(HERE)
 INCLUDE = os.path.join(os.path.dirname(PKG), "include")
-NAMES = ("correlation_cuda", "resample2d_cuda", "channelnorm_cuda")
+NAMES = ("correlation_cuda", "resample2d_cuda", "channelnorm_cuda", "fn2b200_ops")
 SUFFIX = sysconfig.get_config_var("EXT_SUFFIX") or ".so"
 
 
@@ -65,7 +66,7 @@ def build(force=False):
             raise RuntimeError("%s: libstdc++ was linked statically into the extension (compiler %s); use the system g++" % (name, cxx))
         os.replace(target(name) + ".tmp", target(name))
         return target(name)
-    with ThreadPoolExecutor(max_workers=3) as ex:
+    with ThreadPoolExecutor(max_workers=len(NAMES)) as ex:
         outs = list(ex.map(one, NAMES))
     open(stamp, "w").write(digest)
     return outs

@@ -3,8 +3,6 @@
 #include "ext_common.h"
 using namespace fn2ext;
 
-static int dtype16(const at::Tensor &t) { return t.scalar_type() == at::kHalf ? 1 : (t.scalar_type() == at::kBFloat16 ? 2 : 0); }
-
 int channelnorm_cuda_forward(at::Tensor &input1, at::Tensor &output, int norm_deg) {
     TORCH_CHECK(input1.is_cuda() && output.is_cuda() && output.is_contiguous(), "CUDA tensors, contiguous output required");
     TORCH_CHECK(input1.scalar_type() == output.scalar_type(), "input1 / output dtype mismatch");

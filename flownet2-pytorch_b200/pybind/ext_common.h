@@ -26,5 +26,7 @@ inline void *stream_of(const at::Tensor &t) { return at::cuda::getCurrentCUDAStr
 inline at::Tensor scratch(size_t bytes, const at::Tensor &like) {
     return at::empty({(int64_t)(bytes ? bytes : 16)}, like.options().dtype(at::kByte));
 }
+// the C ABI's dtype code of a 16-bit tensor (1 = fp16, 2 = bf16), 0 for anything else
+inline int dtype16(const at::Tensor &t) { return t.scalar_type() == at::kHalf ? 1 : (t.scalar_type() == at::kBFloat16 ? 2 : 0); }
 
 }  // namespace fn2ext

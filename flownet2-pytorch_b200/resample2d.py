@@ -5,35 +5,23 @@ non-contiguous view (no ``.contiguous()`` copy, :48), outputs are not zero-fille
 overwritten (:18), and the image-gradient buffer is zeroed inside the C-ABI call on the same stream.
 """
 import torch
-from torch.autograd import Function
-from torch.autograd.function import once_differentiable
 from torch.nn.modules.module import Module
 
 from . import functional as F2
+from .ops import fn2b200
 
 
-class Resample2dFunction(Function):
+def resample2d(input1, input2, kernel_size=1, bilinear=True):
+    """torch.ops.fn2b200.resample2d_forward (differentiable; the output in input1's dtype)."""
+    F2._require_cuda(input1, input2)
+    out = fn2b200.resample2d_forward(input1, input2, kernel_size, bilinear)
+    return out if input1.dtype == torch.float32 else out.to(input1.dtype)
 
-    @staticmethod
-    def forward(ctx, input1, input2, kernel_size=1, bilinear=True):
-        ctx.save_for_backward(input1, input2)
-        ctx.kernel_size = kernel_size
-        ctx.bilinear = bilinear
-        out = F2.resample2d_forward(input1, input2, kernel_size, bilinear)
-        return out if input1.dtype == torch.float32 else out.to(input1.dtype)
 
-    @staticmethod
-    @once_differentiable
-    def backward(ctx, grad_output):
-        input1, input2 = ctx.saved_tensors
-        need1, need2 = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
-        g1, g2 = F2.resample2d_backward(input1, input2, grad_output, ctx.kernel_size, ctx.bilinear,
-                                        need1=need1, need2=need2)
-        if g1 is not None and g1.dtype != input1.dtype:
-            g1 = g1.to(input1.dtype)
-        if g2 is not None and g2.dtype != input2.dtype:
-            g2 = g2.to(input2.dtype)
-        return g1, g2, None, None
+class Resample2dFunction(object):
+    """reference: resample2d.py:7-38 -- ``Resample2dFunction.apply(input1, input2, kernel_size, bilinear)``, forwarded to
+    the operator (``resample2d``)."""
+    apply = forward = staticmethod(resample2d)
 
 
 class Resample2d(Module):
@@ -45,7 +33,7 @@ class Resample2d(Module):
         self.bilinear = bilinear
 
     def forward(self, input1, input2):
-        return Resample2dFunction.apply(input1, input2, self.kernel_size, self.bilinear)
+        return resample2d(input1, input2, self.kernel_size, self.bilinear)
 
     def extra_repr(self):
         return "kernel_size=%d, bilinear=%s" % (self.kernel_size, self.bilinear)

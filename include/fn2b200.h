@@ -35,6 +35,9 @@
  *   - The library keeps no mutable global state (bar a launch counter): every call is re-entrant and thread-safe
  *     (nn.DataParallel calls these from one Python thread per GPU, main.py:200).
  *   - Outputs are fully overwritten; no pre-zeroing is required except where noted.
+ *   - No entry point synchronises, allocates device memory or keeps state between calls (scratch is always a
+ *     caller-provided workspace; fills are cudaMemsetAsync on `stream`), so every call can be captured into a CUDA
+ *     graph on a capturing stream.
  */
 #ifndef FN2B200_H_
 #define FN2B200_H_
