@@ -37,12 +37,16 @@ __device__ __forceinline__ float2 load_flow(const FlowSrc &f, int b, int y, int 
     float l1h = hs - (float)h1, l0h = 1.f - l1h, l1w = ws - (float)w1, l0w = 1.f - l1w;
     const float *r = q + (long)h1 * f.fw + w1;
     float2 out;
-    // torch's upsample_bilinear2d: h0 * (w0 * v00 + w1 * v01) + h1 * (w0 * v10 + w1 * v11)
-    out.x = l0h * (l0w * (__ldg(r) * f.mul) + l1w * (__ldg(r + wp) * f.mul)) +
-            l1h * (l0w * (__ldg(r + hp) * f.mul) + l1w * (__ldg(r + hp + wp) * f.mul));
-    r += plane;
-    out.y = l0h * (l0w * (__ldg(r) * f.mul) + l1w * (__ldg(r + wp) * f.mul)) +
-            l1h * (l0w * (__ldg(r + hp) * f.mul) + l1w * (__ldg(r + hp + wp) * f.mul));
+    // torch's upsample_bilinear2d: h0 * (w0 * v00 + w1 * v01) + h1 * (w0 * v10 + w1 * v11).  Explicit mul / fma (the
+    // contraction the compiler chose for the plain expression) so that every kernel variant computes the same flow
+    // bits: a 1-ulp change of the flow can move a tap's floor.
+    const auto lerp = [&](const float *p) {
+        const float row0 = __fmaf_rn(l0w, __fmul_rn(__ldg(p), f.mul), __fmul_rn(l1w, __fmul_rn(__ldg(p + wp), f.mul)));
+        const float row1 = __fmaf_rn(l0w, __fmul_rn(__ldg(p + hp), f.mul), __fmul_rn(l1w, __fmul_rn(__ldg(p + hp + wp), f.mul)));
+        return __fmaf_rn(l0h, row0, __fmul_rn(l1h, row1));
+    };
+    out.x = lerp(r);
+    out.y = lerp(r + plane);
     return out;
 }
 
