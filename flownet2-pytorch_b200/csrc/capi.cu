@@ -128,23 +128,6 @@ static int corr_backward(const char *who, const float *in1, const float *in2, co
     }
 }
 
-// FN2B200_RESAMPLE selects the Resample2d kernel family: "tile" (default; 2-D tiles, L1-cached gathers) or "row"
-// (round 1: one CTA = 256 pixels of a row; kept as the comparison point).
-enum { RS_TILE = 0, RS_ROW = 2 };
-static int rs_family() {
-    const char *e = getenv("FN2B200_RESAMPLE");
-    if (e && (e[0] == 'r' || e[0] == 'R' || e[0] == 'g' || e[0] == 'G')) return RS_ROW;
-    return RS_TILE;
-}
-// FN2B200_RS_BWD selects how the tile backward scatters the image gradient: "vec" (default: one 16-byte reduction per
-// tap into a pixel-interleaved scratch, then a transpose; needs C <= 3 and the workspace) or "planar" (one scalar
-// reduction per tap and channel straight into the gradient).
-static int rs_scatter() {
-    const char *e = getenv("FN2B200_RS_BWD");
-    if (e && (e[0] == 'p' || e[0] == 'P')) return 1;
-    return 2;
-}
-
 }  // namespace fn2
 
 using namespace fn2;
@@ -287,11 +270,8 @@ int fn2b200_resample2d_forward(const float *img, const int64_t *istride, const f
     if (B == 0) return 0;
     if (!img || !flow || !out) return fail(FN2B200_ENULL, "resample2d_forward: null pointer");
     if ((rc = bind_device_of(flow))) return rc;
-    const int fam = rs_family();
     FlowSrc fs = {flow, H, W, 0, 1.f};
     WarpOut o = {out, C, -1, 0, 0, -1, -1, -1, 1.f};
-    if (fam == RS_ROW)
-        return resample2d_forward(img, istride, flow, out, B, C, iH, iW, H, W, bilinear, (cudaStream_t)stream);
     return resample2d_forward_tile(img, istride, nullptr, nullptr, fs, o, B, C, H, W, bilinear, (cudaStream_t)stream);
 }
 
@@ -412,9 +392,7 @@ int fn2b200_warp_concat_backward_up(const float *x, const int64_t *xstride, int 
 
 size_t fn2b200_resample2d_backward_workspace(const int64_t *istride, int B, int C, int iH, int iW, int H, int W) {
     if (!istride || B <= 0 || C <= 0 || C > 3 || H <= 0 || W <= 0) return 0;
-    (void)H; (void)W;
-    if (rs_family() == RS_TILE && rs_scatter() == 2) return resample2d_backward_workspace_bytes(B, iH, iW);
-    return 0;
+    return resample2d_backward_workspace_bytes(B, iH, iW);
 }
 
 int fn2b200_resample2d_backward_ws(const float *img, const int64_t *istride, const float *flow,
@@ -428,20 +406,9 @@ int fn2b200_resample2d_backward_ws(const float *img, const int64_t *istride, con
     if (!img || !flow || !gout) return fail(FN2B200_ENULL, "resample2d_backward: null pointer");
     if (!gimg && !gflow) return 0;
     if ((rc = bind_device_of(flow))) return rc;
-    cudaStream_t st = (cudaStream_t)stream;
-    const int fam = rs_family();
-    const bool ws_ok = workspace && workspace_bytes >= resample2d_backward_workspace_bytes(B, iH, iW) &&
-                       !(reinterpret_cast<uintptr_t>(workspace) & 15);
     // zero_grad_input1 == 0: the caller zero-filled grad_input1 and expects accumulation into it (resample2d.py:31)
-    int scatter = fam == RS_ROW ? 1 : rs_scatter();
-    if (scatter == 2 && !(ws_ok && C <= 3)) scatter = 1;
-    if (gimg && zero_grad_input1 && scatter != 2) {          // scatter 2 overwrites grad_input1 from its scratch
-        cudaError_t e = cudaMemsetAsync(gimg, 0, sizeof(float) * (size_t)B * C * iH * iW, st);
-        if (e != cudaSuccess) return fail((int)e, "resample2d_backward: memset failed (%s)", cudaGetErrorString(e));
-    }
-    if (fam == RS_ROW) return resample2d_backward(img, istride, flow, gout, gimg, gflow, B, C, iH, iW, H, W, st);
-    return resample2d_backward_tile(img, istride, flow, gout, gimg, gflow, workspace, scatter, !zero_grad_input1, B, C, iH, iW,
-                                    H, W, st);
+    return resample2d_backward_tile(img, istride, flow, gout, gimg, gflow, workspace, workspace_bytes, zero_grad_input1, B,
+                                    C, iH, iW, H, W, (cudaStream_t)stream);
 }
 
 int fn2b200_channelnorm_forward(const float *in, float *out, int B, int C, int H, int W,

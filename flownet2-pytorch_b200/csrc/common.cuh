@@ -122,11 +122,6 @@ int channelnorm_backward(const float *in, const float *out, const float *gout, f
 int channelnorm_forward_half(const void *in, void *out, int B, int C, int H, int W, int dtype, cudaStream_t st);
 int channelnorm_backward_half(const void *in, const void *out, const void *gout, void *gin, int B, int C, int H,
                               int W, int dtype, cudaStream_t st);
-int resample2d_forward(const float *img, const int64_t *istride, const float *flow, float *out,
-                       int B, int C, int iH, int iW, int H, int W, int bilinear, cudaStream_t st);
-int resample2d_backward(const float *img, const int64_t *istride, const float *flow,
-                        const float *gout, float *gimg, float *gflow, int B, int C, int iH, int iW,
-                        int H, int W, cudaStream_t st);
 
 // Where a kernel gets its flow from.  mode 0: a full-resolution [B,2,H,W] tensor.  mode 1 / 2: a quarter-resolution
 // [B,2,fh,fw] tensor (H = 4 fh, W = 4 fw) that is multiplied by `mul` and upsampled x4 on the fly --
@@ -155,14 +150,15 @@ struct WarpOut {
     int ch_x, n_x, ch_warped, ch_flow, ch_fnorm, ch_dnorm;
     float flow_div;
 };
-// 2-D tile kernels (resample2d_tile.cu): any strides, any C; `scatter` = 1 planar scalar reductions, 2 vector reductions
-// into the pixel-interleaved scratch of resample2d_backward_workspace_bytes() (zero-filled inside the call, transposed
-// afterwards; C <= 3).
+// 2-D tile kernels (resample2d_tile.cu): any strides, any C.  The backward scatters the image gradient with vector
+// reductions into the pixel-interleaved scratch (zero-filled inside the call, transposed afterwards) when C <= 3 and
+// `workspace` is 16-byte aligned and holds resample2d_backward_workspace_bytes(); otherwise with planar scalar
+// reductions into gimg.  zero_gimg == 0: the gradient is added to what gimg holds.
 int resample2d_forward_tile(const float *img1, const int64_t *is1, const float *img0, const int64_t *is0,
                             const FlowSrc &fs, const WarpOut &o, int B, int C, int H, int W, int bilinear, cudaStream_t st);
 int resample2d_backward_tile(const float *img, const int64_t *istride, const float *flow, const float *gout, float *gimg,
-                             float *gflow, void *workspace, int scatter, int accumulate, int B, int C, int iH, int iW,
-                             int H, int W, cudaStream_t st);
+                             float *gflow, void *workspace, size_t workspace_bytes, int zero_gimg, int B, int C, int iH,
+                             int iW, int H, int W, cudaStream_t st);
 size_t resample2d_backward_workspace_bytes(int B, int iH, int iW);
 int resample2d_backward_finish(const float *T, float *gimg, int accumulate, int B, int C, int iH, int iW, cudaStream_t st,
                                long gimg_bstride = 0);

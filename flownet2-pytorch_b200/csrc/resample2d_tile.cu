@@ -8,25 +8,27 @@
 // Why tiles: round 1's kernels mapped a CTA to 256 consecutive pixels of ONE row.  With a sigma = 4 px flow the taps
 // of such a CTA spread over ~30 image rows, every 32-byte sector fetched for one tap is used once and the kernel ran
 // at the L2->SM crossbar ceiling (0.51 GB moved for 0.117 GB of algorithmic traffic, 9.3 TB/s).  A CTA that owns a
-// 32 x (8 PY) pixel tile touches (32 + 2h) x (8 PY + 2h) pixels of the image instead: the sectors it pulls are reused
+// 32 x 32 pixel tile touches (32 + 2h) x (32 + 2h) pixels of the image instead: the sectors it pulls are reused
 // by its other threads out of L1 (the CTAs co-resident on an SM are x-neighbours and share their halos too).
 // What bounds it is the L1 data pipe (a warp-wide tap load touches many lines).  A TMA-staged shared-memory box per
 // CTA moves the same bytes, but flow read -> box placement -> TMA -> gather serialise inside a CTA and large boxes leave
 // few CTAs per SM; it was dropped, as was,
 // for the backward, accumulation in a shared-memory box (below).
 //
-// Thread (lx = tid & 31, ly = tid >> 5) owns pixels (tx0 + lx, ty0 + ly + 8 j), j < PY: flow reads and output stores
-// are 128-byte coalesced rows, the PY pixels give 4 C PY independent gathers in flight per thread.
+// Thread (lx = tid & 31, ly = tid >> 5) owns pixels (tx0 + lx, ty0 + ly + 8 j), j < RS_PY = 4: flow reads and output
+// stores are 128-byte coalesced rows, the 4 pixels give 16 C independent gathers in flight per thread.
 #include "resample_common.cuh"
 
 namespace fn2 {
+
+constexpr int RS_PY = 4;   // pixel rows per thread of resample2d_fwd_tile / resample2d_bwd_tile
 
 struct ImgView {        // a [*, C, H, W] fp32 view with element strides
     const float *p;
     long sb, sc, sh, sw;
 };
 
-template <int CT, int PY, bool FUSED>
+template <int CT, bool FUSED>
 __global__ void __launch_bounds__(256)
 resample2d_fwd_tile(ImgView im1, ImgView im0, FlowSrc fs, WarpOut o, int C, int H, int W, int tiles_x, int tiles_y,
                     int bilinear) {
@@ -35,16 +37,16 @@ resample2d_fwd_tile(ImgView im1, ImgView im0, FlowSrc fs, WarpOut o, int C, int 
     const int bx = t % tiles_x;
     t /= tiles_x;
     const int by = t % tiles_y, b = t / tiles_y;
-    const int x = bx * 32 + lx, y0 = by * (8 * PY) + ly;
+    const int x = bx * 32 + lx, y0 = by * (8 * RS_PY) + ly;
     if (x >= W) return;
     const int Cn = CT > 0 ? CT : C;
     const long hw = (long)H * W;
     const float *ib = im1.p + (long)b * im1.sb;
     float *ob = o.cat + (long)b * o.cat_channels * hw;
 
-    float dx[PY], dy[PY];
+    float dx[RS_PY], dy[RS_PY];
 #pragma unroll
-    for (int j = 0; j < PY; ++j) {
+    for (int j = 0; j < RS_PY; ++j) {
         const int y = y0 + 8 * j;
         dx[j] = dy[j] = 0.f;
         if (y < H) {
@@ -54,7 +56,7 @@ resample2d_fwd_tile(ImgView im1, ImgView im0, FlowSrc fs, WarpOut o, int C, int 
         }
     }
 #pragma unroll
-    for (int j = 0; j < PY; ++j) {
+    for (int j = 0; j < RS_PY; ++j) {
         const int y = y0 + 8 * j;
         if (y >= H) continue;
         const float xf = (float)x + dx[j], yf = (float)y + dy[j];
@@ -113,15 +115,15 @@ resample2d_fwd_tile(ImgView im1, ImgView im0, FlowSrc fs, WarpOut o, int C, int 
 // Backward.  One kernel: the flow gradient (K7, needs the image taps: gathered as in the forward) and the image
 // gradient (K6, a bilinear scatter of gradOutput).  What bounds the scatter (csrc_test/atomics_bench.cu): an SM retires
 // global reductions at a fixed cost per LANE whatever their width, and round 1 issued 4 taps x C of them per pixel.
-// SC selects how the scatter is done:
-//   1  one red.global.add.f32 per tap and channel into the planar gradient (round 1; any shape)
+// SC selects how the scatter is done (0: no image gradient):
+//   1  one red.global.add.f32 per tap and channel into the planar gradient (any C, no workspace)
 //   2  one red.global.add.v4.f32 per tap into a pixel-interleaved scratch T[b][y][x][4] (C <= 3), transposed into the
 //      planar gradient by resample2d_bwd_finish: 4 lane-operations per pixel instead of 12
 // Accumulating in a shared-memory box per CTA and flushing it with coalesced vector reductions was built and measured
 // too: red.shared.add.f32 compiled to a compare-and-swap loop that retries whenever neighbouring pixels hit the same
 // word, which made it slower than the global reductions: dropped.
 // ---------------------------------------------------------------------------------------------------------------
-template <int CT, int PY, int SC>
+template <int CT, int SC>
 __global__ void __launch_bounds__(256)
 resample2d_bwd_tile(ImgView im, FlowSrc fs, const float *__restrict__ gout, float *__restrict__ gimg,
                     float *__restrict__ T, float *__restrict__ gflow, int C, int iH, int iW, int H, int W, int tiles_x,
@@ -131,14 +133,14 @@ resample2d_bwd_tile(ImgView im, FlowSrc fs, const float *__restrict__ gout, floa
     const int bxi = t % tiles_x;
     t /= tiles_x;
     const int byi = t % tiles_y, b = t / tiles_y;
-    const int x = bxi * 32 + lx, y0 = byi * (8 * PY) + ly;
+    const int x = bxi * 32 + lx, y0 = byi * (8 * RS_PY) + ly;
     const int Cn = CT > 0 ? CT : C;
     const long hw = (long)H * W, ihw = (long)iH * iW;
     const bool xok = x < W;
 
-    float dx[PY], dy[PY];
+    float dx[RS_PY], dy[RS_PY];
 #pragma unroll
-    for (int j = 0; j < PY; ++j) {
+    for (int j = 0; j < RS_PY; ++j) {
         const int y = y0 + 8 * j;
         dx[j] = dy[j] = 0.f;
         if (xok && y < H) {
@@ -153,7 +155,7 @@ resample2d_bwd_tile(ImgView im, FlowSrc fs, const float *__restrict__ gout, floa
     float *gi = (SC == 1 && gimg) ? gimg + (long)b * Cn * ihw : nullptr;
     float *Tb = (SC == 2 && T) ? T + (long)b * ihw * 4 : nullptr;
 #pragma unroll
-    for (int j = 0; j < PY; ++j) {
+    for (int j = 0; j < RS_PY; ++j) {
         const int y = y0 + 8 * j;
         if (!(xok && y < H)) continue;
         const float xf = (float)x + dx[j], yf = (float)y + dy[j];
@@ -428,13 +430,6 @@ resample2d_bwd_finish(const float *__restrict__ T, float *__restrict__ gimg, lon
 // ---------------------------------------------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------------------------------------------
-static int env_int(const char *name, int dflt, int lo, int hi) {
-    const char *e = getenv(name);
-    if (!e || !*e) return dflt;
-    int v = atoi(e);
-    return v < lo ? lo : (v > hi ? hi : v);
-}
-
 static ImgView view_of(const float *p, const int64_t *s) {
     ImgView v = {p, 0, 0, 0, 0};
     if (s) { v.sb = s[0]; v.sc = s[1]; v.sh = s[2]; v.sw = s[3]; }
@@ -444,28 +439,23 @@ static ImgView view_of(const float *p, const int64_t *s) {
 int resample2d_forward_tile(const float *img1, const int64_t *is1, const float *img0, const int64_t *is0,
                             const FlowSrc &fs, const WarpOut &o, int B, int C, int H, int W, int bilinear,
                             cudaStream_t st) {
-    const int py = env_int("FN2B200_RS_PY", 4, 1, 4);
-    const int PYc = py >= 4 ? 4 : (py >= 2 ? 2 : 1);
-    const int tiles_x = (W + 31) / 32, tiles_y = (H + 8 * PYc - 1) / (8 * PYc);
+    const int tiles_x = (W + 31) / 32, tiles_y = (H + 8 * RS_PY - 1) / (8 * RS_PY);
     const long ntiles = (long)tiles_x * tiles_y * B;
     if (ntiles >= (1L << 31)) return fail(FN2B200_EINVAL, "resample2d_forward: %ld tiles exceed the grid limit", ntiles);
     const bool fused = o.ch_dnorm >= 0 || o.ch_flow >= 0 || o.ch_fnorm >= 0 || o.ch_x >= 0;
     const ImgView v1 = view_of(img1, is1), v0 = view_of(img0, is0);
     const unsigned grid = (unsigned)ntiles;
-#define FN2_L(CT, PY)                                                                                                    \
+#define FN2_L(CT)                                                                                                        \
     do {                                                                                                               \
-        if (fused) resample2d_fwd_tile<CT, PY, true><<<grid, 256, 0, st>>>(v1, v0, fs, o, C, H, W, tiles_x, tiles_y, bilinear); \
-        else resample2d_fwd_tile<CT, PY, false><<<grid, 256, 0, st>>>(v1, v0, fs, o, C, H, W, tiles_x, tiles_y, bilinear);      \
+        if (fused) resample2d_fwd_tile<CT, true><<<grid, 256, 0, st>>>(v1, v0, fs, o, C, H, W, tiles_x, tiles_y, bilinear); \
+        else resample2d_fwd_tile<CT, false><<<grid, 256, 0, st>>>(v1, v0, fs, o, C, H, W, tiles_x, tiles_y, bilinear);      \
     } while (0)
-#define FN2_C(PY)                                                                                                        \
-    switch (C) {                                                                                                       \
-        case 1: FN2_L(1, PY); break;                                                                                   \
-        case 2: FN2_L(2, PY); break;                                                                                   \
-        case 3: FN2_L(3, PY); break;                                                                                   \
-        default: FN2_L(0, PY); break;                                                                                  \
+    switch (C) {
+        case 1: FN2_L(1); break;
+        case 2: FN2_L(2); break;
+        case 3: FN2_L(3); break;
+        default: FN2_L(0); break;
     }
-    if (PYc == 4) { FN2_C(4) } else if (PYc == 2) { FN2_C(2) } else { FN2_C(1) }
-#undef FN2_C
 #undef FN2_L
     count_launch();
     return check_launch("resample2d_forward");
@@ -473,56 +463,50 @@ int resample2d_forward_tile(const float *img1, const int64_t *is1, const float *
 
 size_t resample2d_backward_workspace_bytes(int B, int iH, int iW) { return (size_t)B * iH * iW * 4 * sizeof(float); }
 
-// scatter: 1 planar scalar reductions, 2 vector reductions into the interleaved scratch (needs workspace, C <= 3)
 int resample2d_backward_tile(const float *img, const int64_t *is, const float *flow, const float *gout, float *gimg,
-                             float *gflow, void *workspace, int scatter, int accumulate, int B, int C, int iH, int iW,
-                             int H, int W, cudaStream_t st) {
-    const int py = env_int("FN2B200_RS_PY", 4, 1, 4);
-    const int PYc = py >= 4 ? 4 : (py >= 2 ? 2 : 1);
-    const int tiles_x = (W + 31) / 32, tiles_y = (H + 8 * PYc - 1) / (8 * PYc);
+                             float *gflow, void *workspace, size_t workspace_bytes, int zero_gimg, int B, int C, int iH,
+                             int iW, int H, int W, cudaStream_t st) {
+    const int tiles_x = (W + 31) / 32, tiles_y = (H + 8 * RS_PY - 1) / (8 * RS_PY);
     const long ntiles = (long)tiles_x * tiles_y * B;
     if (ntiles >= (1L << 31)) return fail(FN2B200_EINVAL, "resample2d_backward: %ld tiles exceed the grid limit", ntiles);
     const unsigned grid = (unsigned)ntiles;
     const ImgView v = view_of(img, is);
     const FlowSrc fs = {flow, H, W, 0, 1.f};
-    if (!gimg) scatter = 0;
-    if (scatter == 2 && (C > 3 || !workspace)) scatter = 1;
-    float *T = nullptr;
-    if (scatter == 2) {
-        T = static_cast<float *>(workspace);
-        cudaError_t e = cudaMemsetAsync(T, 0, resample2d_backward_workspace_bytes(B, iH, iW), st);
-        if (e != cudaSuccess) return fail((int)e, "resample2d_backward: workspace memset failed (%s)", cudaGetErrorString(e));
+    const size_t T_bytes = resample2d_backward_workspace_bytes(B, iH, iW);
+    const bool vec_ok = C <= 3 && workspace && workspace_bytes >= T_bytes && !(reinterpret_cast<uintptr_t>(workspace) & 15);
+    const int scatter = !gimg ? 0 : (vec_ok ? 2 : 1);
+    float *T = scatter == 2 ? static_cast<float *>(workspace) : nullptr;
+    // the scratch starts at 0; the planar scatter adds into gimg, which is zero-filled first unless the caller wants
+    // the gradient added to what it holds.  The vector scatter's finishing transpose stores (or adds) instead.
+    if (scatter == 2 || (scatter == 1 && zero_gimg)) {
+        cudaError_t e = T ? cudaMemsetAsync(T, 0, T_bytes, st) : cudaMemsetAsync(gimg, 0, sizeof(float) * (size_t)B * C * iH * iW, st);
+        if (e != cudaSuccess) return fail((int)e, "resample2d_backward: memset failed (%s)", cudaGetErrorString(e));
     }
-#define FN2_B(CT, PY, SC) resample2d_bwd_tile<CT, PY, SC><<<grid, 256, 0, st>>>(v, fs, gout, gimg, T, gflow, C, iH, iW, H, W, tiles_x, tiles_y)
-#define FN2_BC(PY, SC)                                                                                                   \
+#define FN2_B(CT, SC) resample2d_bwd_tile<CT, SC><<<grid, 256, 0, st>>>(v, fs, gout, gimg, T, gflow, C, iH, iW, H, W, tiles_x, tiles_y)
+#define FN2_BC(SC)                                                                                                       \
     switch (C) {                                                                                                       \
-        case 1: FN2_B(1, PY, SC); break;                                                                               \
-        case 2: FN2_B(2, PY, SC); break;                                                                               \
-        case 3: FN2_B(3, PY, SC); break;                                                                               \
-        default: FN2_B(0, PY, SC); break;                                                                              \
+        case 1: FN2_B(1, SC); break;                                                                                   \
+        case 2: FN2_B(2, SC); break;                                                                                   \
+        case 3: FN2_B(3, SC); break;                                                                                   \
+        default: FN2_B(0, SC); break;                                                                                  \
     }
-// scatter 2 has C <= 3 (see above): no runtime-C instantiation
-#define FN2_BC2(PY)                                                                                                      \
-    switch (C) {                                                                                                       \
-        case 1: FN2_B(1, PY, 2); break;                                                                                \
-        case 2: FN2_B(2, PY, 2); break;                                                                                \
-        default: FN2_B(3, PY, 2); break;                                                                               \
+    if (scatter == 0) {
+        FN2_BC(0)
+    } else if (scatter == 1) {
+        FN2_BC(1)
+    } else {
+        switch (C) {          // C <= 3: no runtime-C instantiation
+            case 1: FN2_B(1, 2); break;
+            case 2: FN2_B(2, 2); break;
+            default: FN2_B(3, 2); break;
+        }
     }
-#define FN2_BS(PY)                                                                                                       \
-    switch (scatter) {                                                                                                 \
-        case 0: FN2_BC(PY, 0) break;                                                                                   \
-        case 1: FN2_BC(PY, 1) break;                                                                                   \
-        default: FN2_BC2(PY) break;                                                                                    \
-    }
-    if (PYc == 4) { FN2_BS(4) } else if (PYc == 2) { FN2_BS(2) } else { FN2_BS(1) }
-#undef FN2_BS
-#undef FN2_BC2
 #undef FN2_BC
 #undef FN2_B
     count_launch();
     int rc = check_launch("resample2d_backward");
     if (rc || scatter != 2) return rc;
-    return resample2d_backward_finish(T, gimg, accumulate, B, C, iH, iW, st);
+    return resample2d_backward_finish(T, gimg, !zero_gimg, B, C, iH, iW, st);
 }
 
 int resample2d_backward_finish(const float *T, float *gimg, int accumulate, int B, int C, int iH, int iW, cudaStream_t st,

@@ -1,5 +1,5 @@
-// resample_common.cuh -- tap arithmetic and flow sources shared by the Resample2d kernels (resample2d.cu: round 1's row
-// kernels; resample2d_tile.cu: 2-D tile kernels, optionally fused with the flow upsample and the concat epilogue).
+// resample_common.cuh -- tap arithmetic and flow sources of the Resample2d kernels (resample2d_tile.cu: 2-D tile
+// kernels, optionally fused with the flow upsample and the concat epilogue).
 #pragma once
 #include "common.cuh"
 

@@ -179,8 +179,8 @@ int fn2b200_resample2d_backward(const float *input1, const int64_t *istride, con
                                 int bilinear, int zero_grad_input1, void *stream);
 
 /*
- * Backward with a caller-provided scratch: fn2b200_resample2d_backward_workspace() returns the bytes needed (0 = C > 3
- * or FN2B200_RS_BWD=planar: scalar reductions straight into grad_input1, what fn2b200_resample2d_backward does), and
+ * Backward with a caller-provided scratch: fn2b200_resample2d_backward_workspace() returns the bytes needed (0 = C > 3:
+ * scalar reductions straight into grad_input1, what fn2b200_resample2d_backward does), and
  * fn2b200_resample2d_backward_ws() is fn2b200_resample2d_backward() plus a 16-byte aligned device workspace of at least
  * that size (NULL is fine when grad_input1 is NULL).  The image gradient is accumulated in the workspace as ONE
  * 16-byte vector reduction per bilinear tap (pixel-interleaved layout [B][iH][iW][4]: 4 lane-operations per pixel

@@ -176,11 +176,6 @@ def test_new_entry_points_validate_arguments_without_gpu():
     assert L.fn2b200_correlation_forward_cat(pf, pf, pf, 440, 0, 0.1, 1, 64, 8, 8, 20, 1, 20, 1, 2, 1, P(0), 0, P(0)) == -1
     assert b"do not fit" in L.fn2b200_last_error()
     assert L.fn2b200_correlation_forward_cat(pf, pf, pf, 473, 32, 0.1, 0, 64, 8, 8, 20, 1, 20, 1, 2, 1, P(0), 0, P(0)) == 0        # B = 0
-    # Resample2d backward scratch: 16 bytes per image pixel for C <= 3, none for C > 3 or the planar scatter
+    # Resample2d backward scratch: 16 bytes per image pixel for C <= 3, none for C > 3
     assert L.fn2b200_resample2d_backward_workspace(st, 2, 3, 8, 8, 8, 8) == 2 * 8 * 8 * 16
     assert L.fn2b200_resample2d_backward_workspace(st, 2, 5, 8, 8, 8, 8) == 0
-    os.environ["FN2B200_RS_BWD"] = "planar"
-    try:
-        assert L.fn2b200_resample2d_backward_workspace(st, 2, 3, 8, 8, 8, 8) == 0
-    finally:
-        del os.environ["FN2B200_RS_BWD"]

@@ -362,25 +362,14 @@ def test_corr_tc_backward_more_than_65535_rows(monkeypatch):
 # ------------------------------------------------------------------------------------------------
 # Resample2d
 # ------------------------------------------------------------------------------------------------
-RS_FAMILIES = {
-    "tile_py1": {"FN2B200_RS_PY": "1"},
-    "tile_py2": {"FN2B200_RS_PY": "2"},
-    "tile_py4": {},
-    "planar_py1": {"FN2B200_RS_PY": "1", "FN2B200_RS_BWD": "planar"},
-    "planar_py2": {"FN2B200_RS_PY": "2", "FN2B200_RS_BWD": "planar"},
-    "planar_py4": {"FN2B200_RS_BWD": "planar"},
-    "row": {"FN2B200_RESAMPLE": "row"},
-}
-
-
 @pytest.mark.parametrize("C", [1, 2, 3, 5])
-@pytest.mark.parametrize("family", list(RS_FAMILIES))
-def test_resample2d(arena, family, C, monkeypatch):
+@pytest.mark.parametrize("scatter", ["vector", "planar"])
+def test_resample2d(arena, scatter, C):
     """An image larger than the flow (iH > H, iW > W) with more samples than the flow (3 > 2), sigma = 6 px so that
     many taps clamp: K7 (forward, flow gradient) clamps with the flow's dims, K6 (image-gradient scatter) with the
-    image's.  The forward, both gradients and the flow gradient alone, against the oracle."""
-    for k, v in RS_FAMILIES[family].items():
-        monkeypatch.setenv(k, v)
+    image's.  The forward, both gradients and the flow gradient alone, against the oracle.  The C ABI backward runs
+    the scatter under test: `vector` hands it the queried workspace (the interleaved scratch when C <= 3), `planar` a
+    NULL workspace of 0 bytes (scalar reductions straight into the gradient)."""
     f = _f2()
     F2, L = f.functional, f._lib.LIB
     B, H, W, iH, iW = 2, 21, 37, 26, 45
@@ -393,10 +382,12 @@ def test_resample2d(arena, family, C, monkeypatch):
     gi, gf = F2.resample2d_backward(imd, fld, gd, out1=arena.out((3, C, iH, iW)), out2=arena.out((B, 2, H, W)))
     none, gf_only = F2.resample2d_backward(imd, fld, gd, need1=False, out2=arena.out((B, 2, H, W)))
     assert none is None
-    # the C ABI with a workspace of exactly the queried size (0 for the planar and row scatters and for C > 3)
+    # the C ABI with the scatter's workspace: exactly the queried size (0 for C > 3), or none
     st = F2._img_strides(imd)
     nws = int(L.fn2b200_resample2d_backward_workspace(st, B, C, iH, iW, H, W))
-    assert (nws > 0) == (family.startswith("tile") and C <= 3)
+    assert (nws > 0) == (C <= 3)
+    if scatter == "planar":
+        nws = 0
     ws = arena.workspace(nws)
     gi_ws, gf_ws = arena.out((B, C, iH, iW)), arena.out((B, 2, H, W))
     assert L.fn2b200_resample2d_backward_ws(_p(imd), st, _p(fld), _p(gd), _p(gi_ws), _p(gf_ws), B, C, iH, iW, H, W, 1, 1, 1,
@@ -404,21 +395,23 @@ def test_resample2d(arena, family, C, monkeypatch):
     arena.check()
     ref = orc.resample2d_forward(img.numpy(), flow.numpy())
     rgi, rgf = orc.resample2d_backward(img.numpy(), flow.numpy(), gout.numpy())
-    assert_close(out.cpu().numpy(), ref, TOL, "%s C=%d forward" % (family, C))
+    assert_close(out.cpu().numpy(), ref, TOL, "%s C=%d forward" % (scatter, C))
     gi_n = gi.cpu().numpy()
-    assert_close(gi_n, rgi, TOL, "%s C=%d image gradient" % (family, C))
-    assert_close(gf.cpu().numpy(), rgf, TOL, "%s C=%d flow gradient" % (family, C))
-    assert_close(gi_ws.cpu().numpy(), rgi[:B], TOL, "%s C=%d image gradient (C ABI)" % (family, C))
+    assert_close(gi_n, rgi, TOL, "%s C=%d image gradient" % (scatter, C))
+    assert_close(gf.cpu().numpy(), rgf, TOL, "%s C=%d flow gradient" % (scatter, C))
+    gi_ws_n = gi_ws.cpu().numpy()
+    assert_close(gi_ws_n, rgi[:B], TOL, "%s C=%d image gradient (C ABI)" % (scatter, C))
     assert (gi_n[B:] == 0).all(), "image-gradient rows beyond the flow batch must be exactly 0"
-    beyond = np.concatenate([gi_n[:B, :, H:].ravel(), gi_n[:B, :, :, W:].ravel()])
-    assert (beyond != 0).any(), "no image-gradient tap beyond the flow's (H, W): the case does not test K6's clamp"
+    for g_n in (gi_n, gi_ws_n):
+        beyond = np.concatenate([g_n[:B, :, H:].ravel(), g_n[:B, :, :, W:].ravel()])
+        assert (beyond != 0).any(), "no image-gradient tap beyond the flow's (H, W): the case does not test K6's clamp"
     # the flow gradient does not depend on whether the image gradient is computed, nor on the scatter
     assert torch.equal(gf, gf_only) and torch.equal(gf, gf_ws)
     # fp64 second opinion of the forward where the semantics coincide (image and flow of one size: grid_sample)
     sub = torch.from_numpy(img.numpy()[:B, :, :H, :W]).double()
     r64 = torch_ref.resample2d(sub, flow.double()).numpy()
     same = F2.resample2d_forward(sub.float().cuda(), fld).cpu().numpy()
-    assert_close(same, r64, TOL, "%s C=%d forward vs fp64" % (family, C))
+    assert_close(same, r64, TOL, "%s C=%d forward vs fp64" % (scatter, C))
 
 
 # ------------------------------------------------------------------------------------------------
@@ -512,12 +505,10 @@ def test_warp_concat_backward_one_cell_flow(arena, C, mode, shape):
     _warp_case(arena, C, mode, "both", "concat", shape, 300 + 10 * C + mode)
 
 
-@pytest.mark.parametrize("py", [1, 2, 4])
 @pytest.mark.parametrize("C", [1, 2, 3, 4, 5])
-def test_warp_concat_forward(arena, C, py, monkeypatch):
-    """The fused forward for C = 1..5 (C >= 4: the runtime-C kernel) and each pixel-rows-per-thread setting, through
-    the bilinear upsample; one output channel that no product owns must keep its sentinel."""
-    monkeypatch.setenv("FN2B200_RS_PY", str(py))
+def test_warp_concat_forward(arena, C):
+    """The fused forward for C = 1..5 (C >= 4: the runtime-C kernel), through the bilinear upsample; one output channel
+    that no product owns must keep its sentinel."""
     F2 = _f2().functional
     B, fh, fw = 2, 5, 9
     H, W = 4 * fh, 4 * fw
@@ -533,7 +524,7 @@ def test_warp_concat_forward(arena, C, py, monkeypatch):
     got = out.cpu().numpy()
     assert (got[:, 3 * C + 3] == SENTINEL).all(), "the unowned channel was written"
     ref[:, 3 * C + 3] = SENTINEL
-    assert_close(got, ref, TOL, "fused forward C=%d py=%d" % (C, py))
+    assert_close(got, ref, TOL, "fused forward C=%d" % C)
     if C > 3:
         with pytest.raises(RuntimeError, match="C=%d > 3" % C):
             F2.warp_concat_backward(x.cuda(), lr.cuda(), torch.zeros(B, nch, H, W, device="cuda"), C=C, upsample="bilinear",

@@ -282,14 +282,14 @@ def test_resample2d_vs_oracle(shape, sigma, C):
 @pytest.mark.parametrize("shape,sigma,C", [((2, 40, 72), 4.0, 3), ((1, 33, 52), 64.0, 3), ((2, 64, 128), 2.0, 2),
                                            ((1, 70, 200), 9.0, 1), ((1, 36, 64), 30.0, 3), ((1, 96, 256), 0.3, 3),
                                            ((1, 21, 45), 5.0, 5), ((2, 19, 30), 3.0, 3)])
-def test_resample2d_kernel_families_vs_oracle(shape, sigma, C, monkeypatch):
-    """Every Resample2d kernel family on the same inputs: 2-D tiles (default; PY = 1, 2, 4 rows per thread; both scatter
-    flavours of the backward: vector reductions into the interleaved scratch, planar scalar reductions) and round 1's
-    row kernels; partial tiles on both axes, C = 1, 2, 3 and the runtime-C path (5).
-    Forward and flow gradient must agree bit for bit across families (same arithmetic); the image gradient (atomic
-    order differs) within 1e-5; everything against the oracle within the 1e-4 contract."""
+def test_resample2d_kernel_families_vs_oracle(shape, sigma, C):
+    """Both image-gradient scatters of the Resample2d backward on the same inputs: vector reductions into the
+    interleaved scratch (the functional path, which hands the library the queried workspace) and planar scalar
+    reductions (the C ABI's workspace-less fn2b200_resample2d_backward); partial tiles on both axes, C = 1, 2, 3 and
+    the runtime-C path (5).  Forward and flow gradient must agree bit for bit across the two runs (same arithmetic);
+    the image gradient (atomic order differs) within 1e-5; everything against the oracle within the 1e-4 contract."""
     f = _f2()
-    F2 = f.functional
+    F2, L = f.functional, f._lib.LIB
     B, H, W = shape
     g = torch.Generator().manual_seed(23)
     img = torch.rand(B, C, H, W, generator=g)
@@ -303,19 +303,24 @@ def test_resample2d_kernel_families_vs_oracle(shape, sigma, C, monkeypatch):
     huge[0, 0, 1, 1] = 3e9                               # saturating float->int conversion (UB in the C oracle)
     huge[0, 1, 2, 2] = -float("inf")
     hud = huge.cuda()
+
+    def backward(scatter, need1=True, need2=True):
+        if scatter == "vector":
+            return F2.resample2d_backward(imd, fld, god, need1=need1, need2=need2)
+        # the workspace-less C ABI entry point: the planar scatter
+        g1, g2 = torch.empty_like(imd) if need1 else None, torch.empty_like(fld) if need2 else None
+        p = [t.data_ptr() if t is not None else None for t in (imd, fld, god, g1, g2)]
+        assert L.fn2b200_resample2d_backward(p[0], F2._img_strides(imd), *p[1:], B, C, H, W, H, W, 1, 1, 1,
+                                             torch.cuda.current_stream().cuda_stream) == 0, L.fn2b200_last_error()
+        return g1, g2
+
     base = {}
-    envs = [("tile", {}), ("tile py1", {"FN2B200_RS_PY": "1"}), ("tile py2 planar", {"FN2B200_RS_PY": "2", "FN2B200_RS_BWD": "planar"}),
-            ("tile py4 planar", {"FN2B200_RS_BWD": "planar"}), ("row", {"FN2B200_RESAMPLE": "row"})]
-    for name, env in envs:
-        for k, v in env.items():
-            monkeypatch.setenv(k, v)
+    for name in ("vector", "planar"):
         out = F2.resample2d_forward(imd, fld)
-        g1, g2 = F2.resample2d_backward(imd, fld, god)
-        of = F2.resample2d_backward(imd, fld, god, need1=False)
-        oi = F2.resample2d_backward(imd, fld, god, need2=False)
+        g1, g2 = backward(name)
+        of = backward(name, need1=False)
+        oi = backward(name, need2=False)
         oh = torch.nan_to_num(F2.resample2d_forward(imd, hud), nan=-1.0)
-        for k in env:
-            monkeypatch.delenv(k)
         assert_close(out.cpu().numpy(), ref, TOL, name + ": resample fwd")
         assert_close(g1.cpu().numpy(), r1, TOL, name + ": resample gImg")
         assert_close(g2.cpu().numpy(), r2, TOL, name + ": resample gFlow")
@@ -327,10 +332,10 @@ def test_resample2d_kernel_families_vs_oracle(shape, sigma, C, monkeypatch):
             assert bool((oh[0, :, 0, 0] == -1.0).all())
         else:
             d = (out - base["out"]).abs().max().item()
-            assert torch.equal(out, base["out"]), "%s: forward differs from the tile kernel by %.3e" % (name, d)
+            assert torch.equal(out, base["out"]), "%s: forward differs from the first run by %.3e" % (name, d)
             assert torch.equal(g2, base["g2"]), name + ": flow gradient differs"
             assert torch.equal(oh, base["oh"]), name + ": NaN / inf / huge flows handled differently"
-            assert_close(g1.cpu().numpy(), base["g1"].cpu().numpy(), 1e-5, name + ": image gradient vs tile kernel")
+            assert_close(g1.cpu().numpy(), base["g1"].cpu().numpy(), 1e-5, name + ": image gradient vs the vector scatter")
 
 
 def test_resample2d_shim_accumulates_into_caller_zeroed_gradient():

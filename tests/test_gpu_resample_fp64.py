@@ -27,7 +27,7 @@ GLOBAL_TOL comes from the first passing run of this file, on an H100 80GB HBM3 (
 30 cases, about 25 s).  The largest values over all cases were:
 
     quantity                      max |d| / (kappa S)   max|d| / max|ref64|
-    forward (every family)        0.433                 1.2e-7
+    forward                       0.433                 1.2e-7
     K7                            0.271                 8.1e-8
     K6                            0.332                 3.9e-7
     fused forward                 0.800                 1.0e-7
@@ -61,9 +61,9 @@ The fused backward has one more: an adjoint that drops tile (0, 0)'s partial for
 neighbours must be rejected on those cells.  The catalogue also reaches the fused kernels: full-resolution edge flows in
 mode 0, and through the nearest upsample in mode 2 (each cell holds its top-left pixel's edge flow / 4, exact).
 
-Bit-for-bit invariances: the forward is identical in every family and PY; the Resample2d flow gradient is identical
-across the tile PYs, scatter modes and need1; the warp-concat flow gradient is identical in a repeat call, with and
-without the image gradient, and for a sample alone and inside a batch.  Image gradients go through atomics and are
+Bit-for-bit invariances: the Resample2d forward is identical in both runs (one per scatter); the Resample2d flow
+gradient is identical across the two scatters and need1; the warp-concat flow gradient is identical in a repeat call,
+with and without the image gradient, and for a sample alone and inside a batch.  Image gradients go through atomics and are
 only bounded.
 """
 import ctypes
@@ -78,13 +78,9 @@ from guarded import SENTINEL, Arena
 pytestmark = pytest.mark.gpu
 P = ctypes.c_void_p
 GLOBAL_TOL = 1e-5
-FAMILIES = {
-    "tile_py1": {"FN2B200_RS_PY": "1"}, "tile_py2": {"FN2B200_RS_PY": "2"}, "tile_py4": {},
-    "planar_py1": {"FN2B200_RS_PY": "1", "FN2B200_RS_BWD": "planar"},
-    "planar_py2": {"FN2B200_RS_PY": "2", "FN2B200_RS_BWD": "planar"},
-    "planar_py4": {"FN2B200_RS_BWD": "planar"}, "row": {"FN2B200_RESAMPLE": "row"},
-}
-ENV = ("FN2B200_RS_PY", "FN2B200_RS_BWD", "FN2B200_RESAMPLE")
+# the Resample2d image-gradient scatter, chosen by the workspace the backward is handed: the queried size (vector
+# reductions into the interleaved scratch) or none (planar scalar reductions)
+SCATTERS = ("vector", "planar")
 STATS = {}
 # edge of the catalogue -> (the output that shows it, the variant of the restatement that is wrong only there)
 CONTROLS = {
@@ -142,22 +138,15 @@ def _rejects(x, ref, E, mask):
     return bool(((x.double() - ref).abs() > E + r64.ETA)[mask].any())
 
 
-def _set_family(monkeypatch, fam):
-    for k in ENV:
-        monkeypatch.delenv(k, raising=False)
-    for k, v in FAMILIES[fam].items():
-        monkeypatch.setenv(k, v)
-
-
 # ----------------------------------------------------------------------------------------------------------------
-# Resample2d: every family at tile-boundary geometries, edge flows, negative controls and invariances
+# Resample2d: both scatters at tile-boundary geometries, edge flows, negative controls and invariances
 # ----------------------------------------------------------------------------------------------------------------
 # (B, C, H, W, image batch, iH, iW)
 RS_SHAPES = [(1, 1, 1, 1, 2, 3, 4), (3, 2, 7, 31, 3, 7, 31), (1, 3, 9, 32, 2, 12, 40), (3, 4, 8, 33, 4, 10, 35),
              (1, 5, 33, 95, 2, 40, 100), (3, 3, 31, 17, 4, 31, 20), (1, 2, 15, 64, 1, 17, 66)]
 
 
-def _rs_calls(L, img, flow, gout, arena):
+def _rs_calls(L, img, flow, gout, scatter, arena):
     B, C, H, W = gout.shape
     iB, _, iH, iW = img.shape
     st = _strides(img)
@@ -167,7 +156,7 @@ def _rs_calls(L, img, flow, gout, arena):
         assert L.fn2b200_resample2d_forward(_p(img), st, _p(flow), _p(o), B, C, iH, iW, H, W, 1, bil, _st()) == 0, \
             L.fn2b200_last_error()
         r["fwd", bil] = o
-    nws = int(L.fn2b200_resample2d_backward_workspace(st, B, C, iH, iW, H, W))
+    nws = int(L.fn2b200_resample2d_backward_workspace(st, B, C, iH, iW, H, W)) if scatter == "vector" else 0
     ws = arena.workspace(nws)
     gi, gf = arena.out((B, C, iH, iW)), arena.out((B, 2, H, W))
     assert L.fn2b200_resample2d_backward_ws(_p(img), st, _p(flow), _p(gout), _p(gi), _p(gf), B, C, iH, iW, H, W, 1, 1, 1,
@@ -181,7 +170,7 @@ def _rs_calls(L, img, flow, gout, arena):
 
 
 @pytest.mark.parametrize("B,C,H,W,iB,iH,iW", RS_SHAPES, ids=["x".join(map(str, s)) for s in RS_SHAPES])
-def test_resample2d_fp64(B, C, H, W, iB, iH, iW, monkeypatch, record_property):
+def test_resample2d_fp64(B, C, H, W, iB, iH, iW, record_property):
     L = _f2()._lib.LIB
     g = torch.Generator().manual_seed(1000 + 7 * H + W)
     img = (torch.rand(iB, C, iH, iW, generator=g) - 0.5).cuda()
@@ -193,25 +182,22 @@ def test_resample2d_fp64(B, C, H, W, iB, iH, iW, monkeypatch, record_property):
     bwd = r64.backward(img, flow, gout)
     Ef, E7, E6 = r64.gamma(7) * Sf, r64.gamma(C + 5) * bwd["S_K7"], r64.gamma(bwd["n_K6"] + 5) * bwd["S_K6"]
     first, stats = None, {}
-    for fam in FAMILIES:
-        _set_family(monkeypatch, fam)
-        py = 1 if fam == "row" else int(FAMILIES[fam].get("FN2B200_RS_PY", "4"))
-        r = _rs_calls(L, img, flow, gout, Arena())
-        wt = lambda i, py=py, fam=fam: fam + ": " + _where_tile(i, py)          # noqa: E731
-        _check(r["fwd", 1], fwd, Ef, "forward %s" % fam, wt, stats)
-        assert torch.equal(r["fwd", 0].double(), near), "%s: nearest forward differs from the restatement" % fam
-        _check(r["gflow"], bwd["gflow"], E7, "K7 %s" % fam, wt, stats)
-        _check(r["gimg"], bwd["gimg"], E6, "K6 %s" % fam, wt, stats)
+    for sc in SCATTERS:
+        r = _rs_calls(L, img, flow, gout, sc, Arena())
+        wt = lambda i, sc=sc: sc + ": " + _where_tile(i, 4)                     # noqa: E731
+        _check(r["fwd", 1], fwd, Ef, "forward %s" % sc, wt, stats)
+        assert torch.equal(r["fwd", 0].double(), near), "%s: nearest forward differs from the restatement" % sc
+        _check(r["gflow"], bwd["gflow"], E7, "K7 %s" % sc, wt, stats)
+        _check(r["gimg"], bwd["gimg"], E6, "K6 %s" % sc, wt, stats)
         # pixels no contribution reaches are exactly 0
-        assert bool((r["gimg"][(bwd["n_K6"] == 0).expand_as(r["gimg"])] == 0).all()), fam + ": untouched gradient != 0"
-        assert torch.equal(r["gflow"], r["gflow_only"]), fam + ": the flow gradient depends on need1"
+        assert bool((r["gimg"][(bwd["n_K6"] == 0).expand_as(r["gimg"])] == 0).all()), sc + ": untouched gradient != 0"
+        assert torch.equal(r["gflow"], r["gflow_only"]), sc + ": the flow gradient depends on need1"
         if first is None:
             first = r
         else:
             assert torch.equal(r["fwd", 1], first["fwd", 1]) and torch.equal(r["fwd", 0], first["fwd", 0]), \
-                fam + ": forward bits differ from tile_py1"
-            if fam.startswith(("tile", "planar")):
-                assert torch.equal(r["gflow"], first["gflow"]), fam + ": flow gradient bits differ from tile_py1"
+                sc + ": forward bits differ from the first run"
+            assert torch.equal(r["gflow"], first["gflow"]), sc + ": flow gradient bits differ from the vector scatter's"
     # negative controls, each judged only at the pixels whose coordinate on that axis is the control's edge, with the
     # wrong variant applied to that axis alone
     hits = r64.edge_hits(flow)
