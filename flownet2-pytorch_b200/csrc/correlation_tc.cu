@@ -316,16 +316,16 @@ corr_fwd_tc_kernel(const __grid_constant__ CUtensorMap m1h, const __grid_constan
 //   gI2[c, q] = 1/C sum_p G2[q, p] f1[c, p],   G2[q, p] = gO[(q - p), p]
 // per parity class: D[128 tile px][C] += A[128][144] * B[144 halo px][C] over the halo-row units, accumulated in
 // registers (warpgroup wg: tile pixels [64 wg, 64 wg + 64), an m64 x nC fragment) for the whole tile.
-//   A = the banded gradOutput matrix, built per unit by the warpgroup's own threads straight from the fp32 gradOutput
-//       planes (bf16 hi/lo split on the fly) into an MN-major SW128 layout [k][64 pixels] (two buffers per warpgroup,
-//       so that building unit u + 1 overlaps the last wgmma group of unit u, and each warpgroup's building overlaps
-//       the other's MMAs);
+//   A = the banded gradOutput matrix, built per unit by a builder warpgroup straight from the fp32 gradOutput planes
+//       (bf16 hi/lo split on the fly) into an MN-major SW128 layout [k][64 pixels], two buffers per MMA warpgroup
+//       handed over through mbarriers (a_full: built, a_empty: the wgmmas that read it are complete), so that the
+//       builders load and build up to two units ahead of the MMAs and across the MMA warpgroups' gradient stores;
 //   B = the other input's halo chunk from the prepass copy ([pixel][channel] bf16 = MN-major operand), one ring slot =
 //       hi OR lo of a K-group (48 halo pixels) x all channel blocks;
-//   3 products (hi*hi, lo*hi | hi*lo) per k-step, N = C <= 256 per instruction.
-// Two threads per tile pixel build A: halo rows {2 hp, 2 hp + 1} x all 21 displacements each.  Loads stay coalesced
-// (lanes = pixels, one displacement plane per instruction); the band positions a pixel row writes are the same for
-// every unit, so the zero columns of A are written ONCE at kernel start and the scatter offsets live in registers.
+//   3 products (hi*hi, lo*hi | hi*lo) per k-step, N = C per instruction (two n128 halves at C = 256).
+// One builder thread per tile pixel: all 4 halo rows x 21 displacements of the unit.  Loads stay coalesced (lanes =
+// pixels, one displacement plane per instruction); the band positions a pixel writes are the same for every unit, so
+// the zero columns of A are written ONCE at kernel start.
 // ------------------------------------------------------------------------------------------------
 constexpr int TB_AHL = TC_N * 128;                 // 18432 B: hi (or lo) of a warpgroup's A, [k][64 pixels] (MN-major, SW128)
 constexpr int TB_ASTG = 2 * TB_AHL;                // hi + lo
@@ -336,18 +336,34 @@ __host__ __device__ constexpr uint32_t tb_a_offset(uint32_t p, uint32_t k) {
     return k * 128u + ((((p >> 3) ^ (k & 7u))) << 4) + (p & 7u) * 2u;
 }
 constexpr int TB_MAXBST = 6;
-constexpr int TB_NBAR = 2 * TB_MAXBST;
+// B ring full / empty, then A full [warpgroup][buffer], A empty [warpgroup][buffer]
+constexpr int TB_NBAR = 2 * TB_MAXBST + 2 * 2 * TB_NAST;
 // B staging: the unit's 144 K indices in 3 groups of 48 (12 halo columns x 4 rows); one ring slot = the hi (or the lo)
-// copy of one group x ALL channel blocks = up to 4 boxes of 6 KB, so every wgmma covers N = C columns.
+// copy of one group x ALL channel blocks = up to 4 boxes of 6 KB, so one k-step covers N = C columns.
 constexpr int TB_NG = 3, TB_GW = TC_HW / TB_NG, TB_GK = TC_UR * TB_GW;   // 3 groups, 12 columns, 48 K
 constexpr int TB_GBLK = TB_GK * 128;               // 6144 B: one 64-channel block of a group's rows
 constexpr int TB_BSTAGE = 4 * TB_GBLK;             // 24576 B: [<= 4 channel blocks][48 rows x 128 B]
 __host__ __device__ constexpr uint32_t tb_kindex(uint32_t hrl, uint32_t qx) {
     return (qx / TB_GW) * TB_GK + hrl * TB_GW + (qx % TB_GW);
 }
-// warps 0-7: two warpgroups (build A, wgmma, epilogue) with 232 registers a thread (setmaxnreg: the m64 x n256 accumulator
-// alone is 128); warps 8-11: a producer warpgroup lowered to 40 registers, of which warp 8 issues the TMA loads
-constexpr int TB_THREADS = TC_CONSUMERS + 128;
+// A offset of halo row h from that of halo row 0: + 12 h k-rows, and an odd h flips bit 2 of k & 7 (the swizzle)
+__host__ __device__ constexpr uint32_t tb_row_offset(uint32_t ao0, uint32_t h) {
+    return (ao0 ^ ((h & 1u) << 6)) + h * TB_GW * 128u;
+}
+__host__ __device__ constexpr bool tb_row_offsets_hold() {
+    for (uint32_t p = 0; p < 64; ++p)
+        for (uint32_t x = 0; x < TC_HW; ++x)
+            for (uint32_t h = 0; h < TC_UR; ++h)
+                if (tb_a_offset(p, tb_kindex(h, x)) != tb_row_offset(tb_a_offset(p, tb_kindex(0, x)), h)) return false;
+    return true;
+}
+static_assert(tb_row_offsets_hold(), "tb_row_offset must match tb_a_offset");
+// warps 0-7: two MMA warpgroups (wgmma, epilogue); warps 8-11: the builder warpgroup (A); warps 12-15: the producer
+// warpgroup, of which warp 12 issues the TMA loads.  Register budgets (setmaxnreg) fill the 64 K register file: the
+// m64 x n256 accumulator alone is 128 registers, a builder thread holds its unit's 84 gradOutput values.
+constexpr int TB_THREADS = TC_CONSUMERS + 256;
+constexpr int TB_REG_MMA = 168, TB_REG_BUILD = 152, TB_REG_PROD = 24;
+static_assert(128 * (2 * TB_REG_MMA + TB_REG_BUILD + TB_REG_PROD) <= 65536, "register budgets exceed the register file");
 __host__ __device__ constexpr int tb_smem_bytes(int bst) {
     return TB_SMEM_A + bst * TB_BSTAGE + TB_NBAR * 8 + 1024;
 }
@@ -357,7 +373,13 @@ __device__ __forceinline__ void wgmma_bwd(float (&d)[NKB * 32], uint64_t da, uin
 template <> __device__ __forceinline__ void wgmma_bwd<1>(float (&d)[32], uint64_t da, uint64_t db) { wgmma_m64n64k16_mn(d, da, db); }
 template <> __device__ __forceinline__ void wgmma_bwd<2>(float (&d)[64], uint64_t da, uint64_t db) { wgmma_m64n128k16_mn(d, da, db); }
 template <> __device__ __forceinline__ void wgmma_bwd<3>(float (&d)[96], uint64_t da, uint64_t db) { wgmma_m64n192k16_mn(d, da, db); }
-template <> __device__ __forceinline__ void wgmma_bwd<4>(float (&d)[128], uint64_t da, uint64_t db) { wgmma_m64n256k16_mn(d, da, db); }
+// C = 256: two n128 halves (channel blocks 0-1, then 2-3).  ptxas places the operands of one instruction within the
+// kernel-wide register limit, 128 at 512 threads, which an n256 accumulator alone fills.  Each accumulator element still
+// receives the same k16 products in the same order.
+template <> __device__ __forceinline__ void wgmma_bwd<4>(float (&d)[128], uint64_t da, uint64_t db) {
+    wgmma_m64n128k16_mn(*reinterpret_cast<float (*)[64]>(&d[0]), da, db);
+    wgmma_m64n128k16_mn(*reinterpret_cast<float (*)[64]>(&d[64]), da, db + ((2 * TB_GBLK) >> 4));
+}
 
 // Ring slots [b, b + n) that the calling warpgroup does not read: wait for each fill, then release it.  Releasing a
 // slot before its fill has landed would complete the previous phase, and a slot refilled before this warpgroup saw its
@@ -390,6 +412,7 @@ corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constan
     unsigned char *sB = smem + TB_SMEM_A;              // [slot][channel block][48 rows x 128 B] (SW128, MN-major)
     uint64_t *bars = reinterpret_cast<uint64_t *>(sB + bst * TB_BSTAGE);
     uint64_t *b_full = bars, *b_empty = bars + TB_MAXBST;
+    uint64_t *a_full = bars + 2 * TB_MAXBST, *a_empty = a_full + 2 * TB_NAST;
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int Hc = H >> 1, Wc = W >> 1;
@@ -403,6 +426,7 @@ corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constan
         prefetch_tensormap(&m2h); prefetch_tensormap(&m2l);
         prefetch_tensormap(&m1h); prefetch_tensormap(&m1l);
         for (int i = 0; i < TB_MAXBST; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], TC_CONSUMERS); }
+        for (int i = 0; i < 2 * TB_NAST; ++i) { mbar_init(&a_full[i], 64); mbar_init(&a_empty[i], 128); }
         fence_barrier_init();
     }
     // columns of A outside a pixel row's band are zero for every unit: written once, here
@@ -410,10 +434,10 @@ corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constan
     fence_proxy_async();
     __syncthreads();
 
-    if (warp >= TC_CONSUMERS / 32) {
+    if (warp >= TC_CONSUMERS / 32 + 4) {
         // ===================== TMA producer: the other input's halo chunks =====================
-        setmaxnreg_dec<40>();
-        if (warp == TC_CONSUMERS / 32 && lane == 0) {
+        setmaxnreg_dec<TB_REG_PROD>();
+        if (warp == TC_CONSUMERS / 32 + 4 && lane == 0) {
             uint32_t bcount = 0;
             const uint64_t pol = l2_policy_evict_last();
             for (int g = t_begin + blockIdx.x; g < t_end; g += gridDim.x) {
@@ -437,110 +461,145 @@ corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constan
         }
         return;
     }
-    setmaxnreg_inc<232>();
 
+    // warpgroup wg's pixel rows 4 wg .. 4 wg + 3 only meet units wg .. wg + 5: the other unit's A would be all zero.
+    // Builders and MMA warpgroups walk the same tiles and units, so the A buffer of a warpgroup's ucount-th unit is
+    // ucount & 1, in its (ucount >> 1)-th use.
+    if (warp >= TC_CONSUMERS / 32) {
+        // ===================== builders: the banded gradOutput matrix A =====================
+        setmaxnreg_inc<TB_REG_BUILD>();
+        // builder warp bw serves MMA warpgroup wg = bw / 2 and covers 4 tile rows x 8 pixels of it (its 32 two-byte
+        // stores of one (halo row, displacement) hit 32 different banks); thread = pixel bp of the warpgroup's 64
+        const int bw = warp - TC_CONSUMERS / 32, wg = bw >> 1;
+        const int bp = (lane >> 3) * TC_TW + (bw & 1) * 8 + (lane & 7);
+        const int bpy = 4 * wg + (bp >> 4), bpx = bp & 15;
+        const int iplane = (int)plane;         // all tensors < 2^31 elements (checked by the C ABI)
+        unsigned char *aw = sA + wg * TB_NAST * TB_ASTG;
+        uint64_t *full = a_full + wg * TB_NAST, *empty = a_empty + wg * TB_NAST;
+        // A offsets of halo row 0 (unit- and tile-invariant, < 2^16), two per register: displacement j in bits
+        // [16 (j & 1), 16 (j & 1) + 16) of ao[j / 2]
+        uint32_t ao[(TC_DS + 1) / 2];
+#pragma unroll
+        for (int j = 0; j < TC_DS; j += 2)
+            ao[j / 2] = tb_a_offset(bp, tb_kindex(0, bpx + j)) | (j + 1 < TC_DS ? tb_a_offset(bp, tb_kindex(0, bpx + j + 1)) << 16 : 0u);
+        uint32_t ucount = 0;
+        for (int g = t_begin + blockIdx.x; g < t_end; g += gridDim.x) {
+            const bool second = both ? (g & 1) : (g >= ntiles);       // gradInput2 tile (block-uniform)
+            const TcTile T = tc_decode(both ? (g >> 1) : (second ? g - ntiles : g), nxt, nyt);
+            const int nbase = T.n * (CAT ? gplanes : TC_DS * TC_DS);
+            // Per-tile address set-up (element offsets fit in 32 bits): the band row of the tile's halo row r (unit
+            // r / 4) starts at off + r * rstep; consecutive displacements are `step` apart; the row is loaded when
+            // tj = r - bpy is a displacement and source row ys0 + r * ystep lies inside the image.
+            int off, rstep, step, ys0, ystep;
+            uint32_t colmask = (1u << TC_DS) - 1u;             // displacements to load (gradInput2: source columns inside the image)
+            {
+                const int yc = T.yc0 + bpy, xc = T.xc0 + bpx;
+                if (!second) {
+                    ys0 = ((yc < Hc) && (xc < Wc)) ? 0 : Hc;       // gO at the output pixel itself
+                    ystep = 0;
+                    off = ((nbase - bpy * TC_DS) * H + (2 * yc + T.py)) * W + (2 * xc + T.px);
+                    step = iplane;                                 // next ti -> next plane
+                    rstep = TC_DS * iplane;                        // next halo row -> tj + 1
+                } else {
+                    ys0 = T.yc0 - TC_DR;                           // source pixel row of halo row 0
+                    ystep = 1;
+                    const int xs0 = T.xc0 - TC_DR + bpx;           // source column for j = 0
+                    off = ((nbase + (TC_DS - 1 + bpy) * TC_DS + (TC_DS - 1)) * H + (2 * ys0 + T.py)) * W + (2 * xs0 + T.px);
+                    step = 2 - iplane;                             // j -> j+1: -1 plane, +2 in x
+                    rstep = 2 * W - TC_DS * iplane;                // next halo row: tj + 1 -> -21 planes, source row + 2
+                    colmask = 0;
+#pragma unroll
+                    for (int j = 0; j < TC_DS; ++j)
+                        if ((unsigned)(xs0 + j) < (unsigned)Wc) colmask |= 1u << j;
+                }
+            }
+            for (int u = wg; u < TC_NU - 1 + wg; ++u, ++ucount) {
+                bool row_ok[TC_UR];
+#pragma unroll
+                for (int h = 0; h < TC_UR; ++h) {
+                    const int r = u * TC_UR + h;
+                    row_ok[h] = ((unsigned)(r - bpy) < (unsigned)TC_DS) && ((unsigned)(ys0 + r * ystep) < (unsigned)Hc);
+                }
+                // CAT with activation: the activations are folded to a bit per displacement (act > 0) before the
+                // gradOutput loads are issued
+                uint32_t pos[TC_UR];
+#pragma unroll
+                for (int h = 0; h < TC_UR; ++h) pos[h] = ~0u;
+                if (CAT && act) {
+                    // all 84 loads issue before the first compare: one round trip per unit, not one per halo row
+                    float a[TC_UR][TC_DS];
+#pragma unroll
+                    for (int h = 0; h < TC_UR; ++h) {
+                        const int base = off + (u * TC_UR + h) * rstep;    // only dereferenced under `ok`
+#pragma unroll
+                        for (int j = 0; j < TC_DS; ++j) {       // predicated, not branched: all loads in flight
+                            const bool ok = row_ok[h] && ((colmask >> j) & 1u);
+                            a[h][j] = ok ? __ldg(act + (base + j * step)) : 1.f;
+                        }
+                    }
+#pragma unroll
+                    for (int h = 0; h < TC_UR; ++h) {
+                        pos[h] = 0u;
+#pragma unroll
+                        for (int j = 0; j < TC_DS; ++j) pos[h] |= a[h][j] > 0.f ? 1u << j : 0u;
+                    }
+                }
+                // the unit's 84 gradOutput loads go out before the wait for the buffer
+                float v[TC_UR][TC_DS];
+#pragma unroll
+                for (int h = 0; h < TC_UR; ++h) {
+                    const int base = off + (u * TC_UR + h) * rstep;
+#pragma unroll
+                    for (int j = 0; j < TC_DS; ++j) {
+                        const bool ok = row_ok[h] && ((colmask >> j) & 1u);
+                        v[h][j] = ok ? __ldg(gout + (base + j * step)) : 0.f;
+                        if (CAT) v[h][j] = ((pos[h] >> j) & 1u) ? v[h][j] : v[h][j] * slope;
+                    }
+                }
+                const int ab = ucount & 1;
+                mbar_wait(&empty[ab], ((ucount >> 1) & 1) ^ 1);   // the wgmmas that read this buffer are complete
+                unsigned char *ah = aw + ab * TB_ASTG, *al = ah + TB_AHL;
+#pragma unroll
+                for (int h = 0; h < TC_UR; ++h)
+#pragma unroll
+                    for (int j = 0; j < TC_DS; ++j) {
+                        const __nv_bfloat16 hv = __float2bfloat16_rn(v[h][j]);
+                        const __nv_bfloat16 lv = __float2bfloat16_rn(v[h][j] - __bfloat162float(hv));
+                        const uint32_t o = tb_row_offset((ao[j / 2] >> (16 * (j & 1))) & 0xFFFFu, h);
+                        *reinterpret_cast<unsigned short *>(ah + o) = __bfloat16_as_ushort(hv);
+                        *reinterpret_cast<unsigned short *>(al + o) = __bfloat16_as_ushort(lv);
+                    }
+                fence_proxy_async();                               // generic-proxy writes -> visible to the tensor core
+                mbar_arrive(&full[ab]);
+            }
+        }
+        return;
+    }
+
+    // ===================== MMA warpgroups: wgmma + epilogue =====================
+    setmaxnreg_inc<TB_REG_MMA>();
     const int wg = warp >> 2, wq = warp & 3;
-    // builder role: pixel bp of the warpgroup's 64 (a warp covers 4 tile rows x 8 pixels: its 32 two-byte stores of
-    // one (halo row, displacement) hit 32 different banks), halo rows {2 hp, 2 hp + 1}
-    const int hp = wq >> 1;
-    const int bp = (lane >> 3) * TC_TW + (wq & 1) * 8 + (lane & 7);
-    const int bpy = 4 * wg + (bp >> 4), bpx = bp & 15;
     // accumulator fragment role: rows 16 wq + lane / 4 (+ 8) of the warpgroup
     const int py_t = 4 * wg + wq, pxa = lane >> 2, q = lane & 3;
-    const int iplane = (int)plane;             // all tensors < 2^31 elements (checked by the C ABI)
-    unsigned char *aw = sA + wg * TB_NAST * TB_ASTG;
+    const uint32_t aw32 = smem_u32(sA + wg * TB_NAST * TB_ASTG);
+    uint64_t *full = a_full + wg * TB_NAST, *empty = a_empty + wg * TB_NAST;
     const float inv_nelems = 1.0f / (float)C;
     uint32_t bcount = 0, ucount = 0;
     for (int g = t_begin + blockIdx.x; g < t_end; g += gridDim.x) {
         const bool second = both ? (g & 1) : (g >= ntiles);           // gradInput2 tile (block-uniform)
         const TcTile T = tc_decode(both ? (g >> 1) : (second ? g - ntiles : g), nxt, nyt);
-        const int nbase = T.n * (CAT ? gplanes : TC_DS * TC_DS);
-        // Per-tile address set-up of the builder pixel (element offsets fit in 32 bits): for unit u the band row of
-        // halo row hrl = 2hp+hh starts at off[hh] + u * dstep; consecutive displacements are `step` apart.
-        int off[2], dstep, step, ystep, tj0[2], ys0[2];
-        uint32_t colmask = 0;                                  // displacements to load (gradInput2: source columns inside the image)
-        {
-            const int yc = T.yc0 + bpy, xc = T.xc0 + bpx;
-            const bool pix_ok = (yc < Hc) && (xc < Wc);
-#pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-                const int hrl = 2 * hp + hh;
-                tj0[hh] = hrl - bpy;                               // tj + 10 at u = 0 (+4 per unit)
-                if (!second) {
-                    ys0[hh] = pix_ok ? 0 : Hc;                     // gO at the output pixel itself
-                    off[hh] = ((nbase + tj0[hh] * TC_DS) * H + (2 * yc + T.py)) * W + (2 * xc + T.px);
-                } else {
-                    ys0[hh] = T.yc0 - TC_DR + hrl;                 // source pixel row at u = 0 (+4 per unit)
-                    const int xs0 = T.xc0 - TC_DR + bpx;           // source column for j = 0
-                    off[hh] = ((nbase + (TC_DS - 1 - tj0[hh]) * TC_DS + (TC_DS - 1)) * H + (2 * ys0[hh] + T.py)) * W +
-                              (2 * xs0 + T.px);
-                    if (hh == 0)
-#pragma unroll
-                        for (int j = 0; j < TC_DS; ++j)
-                            if ((unsigned)(xs0 + j) < (unsigned)Wc) colmask |= 1u << j;
-                }
-            }
-            if (!second) {
-                step = iplane;                                     // next ti -> next plane
-                dstep = TC_UR * TC_DS * iplane;                    // next unit -> tj + 4
-                ystep = 0;
-                colmask = (1u << TC_DS) - 1u;
-            } else {
-                ystep = TC_UR;
-                step = 2 - iplane;                                 // j -> j+1: -1 plane, +2 in x
-                dstep = -TC_UR * TC_DS * iplane + 2 * TC_UR * W;   // next unit: tj + 4 -> -84 planes; source row + 4 -> +8 rows
-            }
-        }
         float acc[C / 2];
 #pragma unroll
         for (int i = 0; i < C / 2; ++i) acc[i] = 0.f;
         wgmma_fence_operands(acc);
-        int prev = -1;                                         // ring slot read by the wgmma group in flight
-        // warpgroup wg's pixel rows 4 wg .. 4 wg + 3 only meet units wg .. wg + 5: the other unit's A would be all zero.
-        // Warpgroup 1 releases unit 0's slots once it has built the A of unit 1, warpgroup 0 unit 6's after its epilogue.
+        int prev = -1, prev_a = -1;                            // ring slot (and A buffer) read by the wgmma group in flight
+        // Warpgroup 1 releases unit 0's slots once the A of unit 1 is built, warpgroup 0 unit 6's after its epilogue.
         if (wg == 1) bcount += 2 * TB_NG;
         for (int u = wg; u < TC_NU - 1 + wg; ++u, ++ucount) {
-            // buffer ucount & 1 was last read by unit ucount - 2, complete since unit ucount - 1's first wait
-            unsigned char *ah = aw + (ucount & 1) * TB_ASTG, *al = ah + TB_AHL;
-#pragma unroll
-            for (int hh = 0; hh < 2; ++hh) {
-                const int tjp = tj0[hh] + u * TC_UR;
-                const bool row_ok = ((unsigned)tjp < (unsigned)TC_DS) && ((unsigned)(ys0[hh] + u * ystep) < (unsigned)Hc);
-                const int base = off[hh] + u * dstep;          // only dereferenced under `ok`
-                // CAT with activation: the activations are reduced to a bit per displacement (act > 0) before the
-                // gradOutput loads, so that 21 values, not 42, are in flight next to the 128-register accumulator
-                uint32_t pos = ~0u;
-                if (CAT && act) {
-                    float a[TC_DS];
-#pragma unroll
-                    for (int j = 0; j < TC_DS; ++j) {           // predicated, not branched: all 21 loads in flight
-                        const bool ok = row_ok && ((colmask >> j) & 1u);
-                        a[j] = ok ? __ldg(act + (base + j * step)) : 1.f;
-                    }
-                    pos = 0u;
-#pragma unroll
-                    for (int j = 0; j < TC_DS; ++j) pos |= a[j] > 0.f ? 1u << j : 0u;
-                }
-                float v[TC_DS];
-#pragma unroll
-                for (int j = 0; j < TC_DS; ++j) {
-                    const bool ok = row_ok && ((colmask >> j) & 1u);
-                    v[j] = ok ? __ldg(gout + (base + j * step)) : 0.f;
-                    if (CAT) v[j] = ((pos >> j) & 1u) ? v[j] : v[j] * slope;
-                }
-#pragma unroll
-                for (int j = 0; j < TC_DS; ++j) {
-                    const __nv_bfloat16 h = __float2bfloat16_rn(v[j]);
-                    const __nv_bfloat16 l = __float2bfloat16_rn(v[j] - __bfloat162float(h));
-                    const uint32_t o = tb_a_offset(bp, tb_kindex(2 * hp + hh, bpx + j));   // unit-invariant
-                    *reinterpret_cast<unsigned short *>(ah + o) = __bfloat16_as_ushort(h);
-                    *reinterpret_cast<unsigned short *>(al + o) = __bfloat16_as_ushort(l);
-                }
-            }
-            fence_proxy_async();                               // generic-proxy writes -> visible to the tensor core
-            named_barrier_sync(1 + wg, 128);                   // the warpgroup's whole A is written
+            const int ab = ucount & 1;
+            mbar_wait(&full[ab], (ucount >> 1) & 1);
             if (u == 1 && wg == 1) tc_skip_slots(b_full, b_empty, bcount - 2 * TB_NG, 2 * TB_NG, bst);
-            const uint32_t ah32 = smem_u32(ah), al32 = smem_u32(al);
+            const uint32_t ah32 = aw32 + ab * TB_ASTG, al32 = ah32 + TB_AHL;
             for (int gr = 0; gr < TB_NG; ++gr)
 #pragma unroll
                 for (int hl = 0; hl < 2; ++hl, ++bcount) {
@@ -557,13 +616,18 @@ corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constan
                     }
                     wgmma_commit();
                     wgmma_wait<1>();
-                    if (prev >= 0) mbar_arrive(&b_empty[prev]);
+                    if (prev >= 0) {
+                        mbar_arrive(&b_empty[prev]);
+                        if (prev_a >= 0) mbar_arrive(&empty[prev_a]);
+                    }
                     prev = s;
+                    prev_a = (gr == TB_NG - 1 && hl == 1) ? ab : -1;   // the unit's last read of its A buffer
                 }
         }
         wgmma_wait<0>();
         wgmma_fence_operands(acc);
         mbar_arrive(&b_empty[prev]);
+        mbar_arrive(&empty[prev_a]);
         // epilogue: fragment rows = tile pixels (py_t, pxa) and (py_t, pxa + 8), columns = channels
         const int yc = T.yc0 + py_t, xc = T.xc0 + pxa;
         const bool ok0 = (yc < Hc) && (xc < Wc), ok1 = (yc < Hc) && (xc + 8 < Wc);
