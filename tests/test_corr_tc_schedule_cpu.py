@@ -82,9 +82,9 @@ def test_fp64_correlation_k1(shape):
     g = torch.Generator().manual_seed(C * 100 + H)
     a, b = torch.randn(B, C, H, W, generator=g).double(), torch.randn(B, C, H, W, generator=g).double()
     prm = (pad, 1, md, 1, s2)
-    out = torch_ref.correlation_k1(a, b, pad, md, s2)
+    out = torch_ref.correlation64(a, b, pad, 1, md, 1, s2)
     go = torch.randn(out.shape, generator=g).double()
-    g1, g2 = torch_ref.correlation_k1_backward(a, b, go, pad, md, s2)
+    g1, g2 = torch_ref.correlation64_backward(a, b, go, pad, 1, md, 1, s2)
     a_, b_ = a.clone().requires_grad_(), b.clone().requires_grad_()
     r = torch_ref.correlation(a_, b_, *prm)
     r.backward(go)
@@ -92,8 +92,8 @@ def test_fp64_correlation_k1(shape):
     for x, ref in ((out, r.detach()), (g1, a_.grad), (g2, b_.grad)):
         assert torch.allclose(x, ref, rtol=1e-12, atol=1e-13)
 
-    S = torch_ref.correlation_k1(a.abs(), b.abs(), pad, md, s2)
-    S1, S2 = torch_ref.correlation_k1_backward(a.abs(), b.abs(), go.abs(), pad, md, s2)
+    S = torch_ref.correlation64(a.abs(), b.abs(), pad, 1, md, 1, s2)
+    S1, S2 = torch_ref.correlation64_backward(a.abs(), b.abs(), go.abs(), pad, 1, md, 1, s2)
     a32, b32, g32 = (t.float().numpy() for t in (a, b, go))
     o = orc.correlation_forward(a32, b32, *prm)
     o1, o2 = orc.correlation_backward(a32, b32, g32, *prm)

@@ -91,7 +91,7 @@ def test_fwd_epilogue_bits(name):
             continue
         n, k = (int(v) for v in np.argwhere(want != got)[0])
         import torch_ref
-        ref = torch_ref.correlation_k1(a[n:n + 1].double(), b[n:n + 1].double(), MD, MD, S2)[0, k]
+        ref = torch_ref.correlation64(a[n:n + 1].double(), b[n:n + 1].double(), MD, 1, MD, 1, S2)[0, k]
         if what == "forward_cat":
             ref = torch.where(ref > 0, ref, ref * SLOPE)
         d = (t[n, k].double() - ref).abs()

@@ -181,8 +181,8 @@ def _check(x, ref, S, K, what, where, stats):
 def _check_fp64(a, b, go, gcat, r, fwd, bwd, stats):
     B, C, H, W = a.shape
     a64, b64, aa, ba = a.double(), b.double(), a.double().abs(), b.double().abs()
-    ref = torch_ref.correlation_k1(a64, b64, MD, MD, S2)
-    S = torch_ref.correlation_k1(aa, ba, MD, MD, S2)
+    ref = torch_ref.correlation64(a64, b64, MD, 1, MD, 1, S2)
+    S = torch_ref.correlation64(aa, ba, MD, 1, MD, 1, S2)
     wf = lambda i: sch.locate_forward(fwd, H, W, *i)                                   # noqa: E731
     _check(r["out"], ref, S, C, "forward", wf, stats)
     _check(r["cat"][:, CH_OFF:CH_OFF + D], torch.where(ref > 0, ref, ref * SLOPE), S, C, "forward_cat", wf, stats)
@@ -191,8 +191,8 @@ def _check_fp64(a, b, go, gcat, r, fwd, bwd, stats):
     del ref, S
     for gname, gout, grads in (("backward", go, r["g", 1, (1, 1)]), ("backward_cat", r["gm"], r["c", 1])):
         g64 = gout.double()
-        refs = torch_ref.correlation_k1_backward(a64, b64, g64, MD, MD, S2)
-        Ss = torch_ref.correlation_k1_backward(aa, ba, g64.abs(), MD, MD, S2)
+        refs = torch_ref.correlation64_backward(a64, b64, g64, MD, 1, MD, 1, S2)
+        Ss = torch_ref.correlation64_backward(aa, ba, g64.abs(), MD, 1, MD, 1, S2)
         for k in range(2):
             wb = lambda i, k=k: "channel %d: %s" % (i[1], sch.locate_backward(bwd, H, W, k, i[0], i[2], i[3]))  # noqa: E731
             _check(grads[k], refs[k], Ss[k], D, "%s grad%d" % (gname, k + 1), wb, stats)
@@ -275,10 +275,10 @@ def test_tc_autograd_and_oracle(C):
     o = orc.correlation_forward(a.numpy(), b.numpy(), *PRM)
     o1, o2 = orc.correlation_backward(a.numpy(), b.numpy(), go.numpy(), *PRM)
     a64, b64 = a.cuda().double(), b.cuda().double()
-    ref = torch_ref.correlation_k1(a64, b64, MD, MD, S2)
-    S = torch_ref.correlation_k1(a64.abs(), b64.abs(), MD, MD, S2)
-    refs = torch_ref.correlation_k1_backward(a64, b64, go.cuda().double(), MD, MD, S2)
-    Ss = torch_ref.correlation_k1_backward(a64.abs(), b64.abs(), go.cuda().double().abs(), MD, MD, S2)
+    ref = torch_ref.correlation64(a64, b64, MD, 1, MD, 1, S2)
+    S = torch_ref.correlation64(a64.abs(), b64.abs(), MD, 1, MD, 1, S2)
+    refs = torch_ref.correlation64_backward(a64, b64, go.cuda().double(), MD, 1, MD, 1, S2)
+    Ss = torch_ref.correlation64_backward(a64.abs(), b64.abs(), go.cuda().double().abs(), MD, 1, MD, 1, S2)
     for x, rr, s, n in ((o, ref, S, C), (o1, refs[0], Ss[0], D), (o2, refs[1], Ss[1], D)):
         assert bool(((torch.from_numpy(x).cuda().double() - rr).abs() <= 2 * (n + 2) * 2.0 ** -24 * s).all())
     assert_close(out[:1].detach().cpu().numpy(), o, 1e-4, "C=%d forward vs oracle" % C)
