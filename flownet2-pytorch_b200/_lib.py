@@ -1,11 +1,15 @@
-"""ctypes binding of libfn2b200.so (the C ABI declared in include/fn2b200.h).
+"""The two native libraries: ``LIB``, the ctypes binding of libfn2b200.so (the C ABI declared in include/fn2b200.h,
+used here for its scalar queries and by the tests of the C ABI), and ``OPS``, the operator library built from
+pybind/fn2b200_ops.cc (torch.ops.fn2b200.* and the host-side glue of every op).
 
-There is NO fallback: if the shared object is missing the import fails loudly, and every entry
+There is NO fallback: if a shared object is missing the import fails loudly, and every entry
 point refuses non-CUDA tensors.  ``FN2B200_AUTOBUILD=1`` (default when nvcc is present) compiles the
-library in-tree on first import; the prebuilt file is what travels to the GPU box.
+libraries in-tree on first import.
 """
 import ctypes
+import importlib.util
 import os
+import sysconfig
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "libfn2b200.so")
@@ -18,14 +22,17 @@ class Fn2B200Error(RuntimeError):
     """A libfn2b200 entry point returned a non-zero status (mirrors the reference's AT_ERROR)."""
 
 
+def _run_build(script):
+    spec = importlib.util.spec_from_file_location("_fn2b200_build", script)
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    mod.build()
+
+
 def _load():
     if not os.path.isfile(LIB_PATH):
         if os.environ.get("FN2B200_AUTOBUILD", "1") == "1":
-            import importlib.util
-            spec = importlib.util.spec_from_file_location("_fn2b200_build", os.path.join(_HERE, "build.py"))
-            mod = importlib.util.module_from_spec(spec)
-            spec.loader.exec_module(mod)
-            mod.build()
+            _run_build(os.path.join(_HERE, "build.py"))
         if not os.path.isfile(LIB_PATH):
             raise ImportError(
                 "libfn2b200.so not found at %s -- build it with `python flownet2-pytorch_b200/build.py` "
@@ -107,6 +114,26 @@ SYMBOLS = (
     "fn2b200_channelnorm_forward", "fn2b200_channelnorm_backward",
     "fn2b200_channelnorm_forward_16", "fn2b200_channelnorm_backward_16",
 )
+
+
+OPS_LIBRARY_PATH = os.path.join(_HERE, "pybind", "fn2b200_ops" + (sysconfig.get_config_var("EXT_SUFFIX") or ".so"))
+
+
+def _load_ops():
+    """pybind/fn2b200_ops.cc, loaded as a Python module: importing it registers the torch.ops.fn2b200 operators, and
+    the module's functions are the host-side glue of every op (what ``functional`` calls)."""
+    if not os.path.isfile(OPS_LIBRARY_PATH) and os.environ.get("FN2B200_AUTOBUILD", "1") == "1":
+        _run_build(os.path.join(_HERE, "pybind", "build_pybind.py"))
+    if not os.path.isfile(OPS_LIBRARY_PATH):
+        raise ImportError("%s not built: run python flownet2-pytorch_b200/pybind/build_pybind.py" % OPS_LIBRARY_PATH)
+    import torch  # noqa: F401  (the module's tensor arguments need torch's bindings)
+    spec = importlib.util.spec_from_file_location("fn2b200_ops", OPS_LIBRARY_PATH)
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    return mod
+
+
+OPS = _load_ops()
 
 
 def check(rc, what):

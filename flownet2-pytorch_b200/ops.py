@@ -1,11 +1,11 @@
 """The layers and the fused ops as PyTorch operators: ``torch.ops.fn2b200.*``.
 
-``pybind/fn2b200_ops.cc`` defines the operators (``TORCH_LIBRARY(fn2b200, m)``) and their CUDA kernels on libfn2b200's
-C ABI; this module loads that library and registers, for each forward, a fake kernel (shapes and dtypes without running
-anything, for torch.compile / torch.export) and an autograd formula whose backward is the matching ``*_backward``
-operator.  Only the gradients in ``ctx.needs_input_grad`` are computed.  The modules and ``*Function`` classes of the
-package (``Correlation``, ``Resample2d``, ``ChannelNorm``, ``fused.CorrelationCat`` / ``WarpConcat`` /
-``FusionConcat``) call these operators, so Dynamo traces them without a graph break, CUDA graphs capture them and
+``pybind/fn2b200_ops.cc`` defines the operators (``TORCH_LIBRARY(fn2b200, m)``) and their CUDA kernels on the host-side
+glue every route shares (``pybind/ext_common.h``); ``_lib`` loads that library, and this module registers, for each
+forward, a fake kernel (shapes and dtypes without running anything, for torch.compile / torch.export) and an autograd
+formula whose backward is the matching ``*_backward`` operator.  Only the gradients in ``ctx.needs_input_grad`` are
+computed.  The modules and ``*Function`` classes of the package (``Correlation``, ``Resample2d``, ``ChannelNorm``,
+``fused.CorrelationCat`` / ``WarpConcat`` / ``FusionConcat``) call these operators, so Dynamo traces them without a graph break, CUDA graphs capture them and
 ``torch.export`` records them as ``fn2b200.*`` calls.  An exported program needs only the operator library:
 ``torch.ops.load_library(flownet2_b200.ops.LIBRARY_PATH)``.
 
@@ -14,36 +14,16 @@ FP32-FMA kernels run) as a second output; autograd saves it and hands it to the 
 pass.  Its size comes from ``fn2b200_correlation_forward_workspace`` at trace time, so a compiled graph is specialised
 on the input sizes and on ``FN2B200_CORR_FWD``.
 """
-import os
-import sysconfig
-
 import torch
 
 from . import functional as F2
-from ._lib import LIB
-
-_HERE = os.path.dirname(os.path.abspath(__file__))
-LIBRARY_PATH = os.path.join(_HERE, "pybind", "fn2b200_ops" + (sysconfig.get_config_var("EXT_SUFFIX") or ".so"))
+from ._lib import LIB, OPS_LIBRARY_PATH as LIBRARY_PATH  # noqa: F401  (importing _lib registers the operators)
 
 #: every operator the library defines
 OPS = ("correlation_forward", "correlation_backward", "correlation_forward_cat", "correlation_backward_cat",
        "resample2d_forward", "resample2d_backward", "channelnorm_forward", "channelnorm_backward",
        "warp_concat_forward", "warp_concat_backward", "fusion_concat", "fusion_concat_backward")
 
-
-def _load():
-    if not os.path.isfile(LIBRARY_PATH) and os.environ.get("FN2B200_AUTOBUILD", "1") == "1":
-        import importlib.util
-        spec = importlib.util.spec_from_file_location("_fn2b200_build_pybind", os.path.join(_HERE, "pybind", "build_pybind.py"))
-        bp = importlib.util.module_from_spec(spec)
-        spec.loader.exec_module(bp)
-        bp.build()
-    if not os.path.isfile(LIBRARY_PATH):
-        raise ImportError("%s not built: run python flownet2-pytorch_b200/pybind/build_pybind.py" % LIBRARY_PATH)
-    torch.ops.load_library(LIBRARY_PATH)
-
-
-_load()
 fn2b200 = torch.ops.fn2b200
 _reg_fake = torch.library.register_fake
 _reg_autograd = torch.library.register_autograd

@@ -1,6 +1,6 @@
 """Build the three pybind extension modules the reference imports by name -- ``correlation_cuda``,
 ``resample2d_cuda``, ``channelnorm_cuda`` (correlation.py:4, resample2d.py:3, channelnorm.py:3) -- and the operator
-library ``fn2b200_ops`` (torch.ops.fn2b200.*, loaded by flownet2_b200.ops) as thin ATen glue over libfn2b200.so's C ABI
+library ``fn2b200_ops`` (torch.ops.fn2b200.*, loaded by flownet2_b200._lib) as thin ATen glue over libfn2b200.so's C ABI
 (g++ only: no device code lives here).
 
     python flownet2-pytorch_b200/pybind/build_pybind.py [--force]

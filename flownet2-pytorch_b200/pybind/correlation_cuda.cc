@@ -7,25 +7,11 @@ int correlation_forward_cuda(at::Tensor &input1, at::Tensor &input2, at::Tensor 
                              at::Tensor &output, int pad_size, int kernel_size, int max_displacement, int stride1,
                              int stride2, int corr_type_multiply) {
     (void)rInput1; (void)rInput2;        // the reference's padded NHWC scratch (:36-41): not needed, left untouched
-    need_cuda_f32(input1, "input1"); need_cuda_f32(input2, "input2"); need_out(output, "output");
-    TORCH_CHECK(input1.dim() == 4 && input1.sizes() == input2.sizes(), "input1 / input2 must be 4-D with equal shapes");
-    int rc;
-    {   // the status is checked (and the exception thrown) after the guard and the temporaries are gone
-        c10::cuda::CUDAGuard guard(input1.device());
-        at::Tensor a = input1.contiguous(), b = input2.contiguous();
-        const int B = a.size(0), C = a.size(1), H = a.size(2), W = a.size(3);
-        int D = 0, oH = 0, oW = 0;
-        rc = fn2b200_correlation_out_shape(C, H, W, pad_size, kernel_size, max_displacement, stride1, stride2, &D, &oH, &oW);
-        if (rc == 0) {
-            output.resize_({B, D, oH, oW});      // :38 (no fill_(0): every element is written)
-            const size_t ws = fn2b200_correlation_forward_workspace(B, C, H, W, pad_size, kernel_size, max_displacement, stride1, stride2);
-            at::Tensor wsb = scratch(ws, a);
-            rc = fn2b200_correlation_forward_ws(a.data_ptr<float>(), b.data_ptr<float>(), output.data_ptr<float>(), B, C, H, W,
-                                                pad_size, kernel_size, max_displacement, stride1, stride2, corr_type_multiply,
-                                                ws ? wsb.data_ptr() : nullptr, ws, stream_of(a));
-        }
-    }
-    check(rc, "correlation_forward");
+    need_cuda_f32(input1, "input1"); need_cuda_f32(input2, "input2"); need_cuda_f32(output, "output");
+    const CorrShape s = corr_shape(input1, input2, pad_size, kernel_size, max_displacement, stride1, stride2);
+    output.resize_({s.B, s.D, s.oH, s.oW});      // :38 (no fill_(0): every element is written)
+    correlation_forward(input1, input2, output, false, 0, 1.0, pad_size, kernel_size, max_displacement, stride1, stride2,
+                        corr_type_multiply);
     return 1;
 }
 
@@ -33,23 +19,13 @@ int correlation_backward_cuda(at::Tensor &input1, at::Tensor &input2, at::Tensor
                               at::Tensor &gradOutput, at::Tensor &gradInput1, at::Tensor &gradInput2, int pad_size,
                               int kernel_size, int max_displacement, int stride1, int stride2, int corr_type_multiply) {
     (void)rInput1; (void)rInput2;
-    need_cuda_f32(input1, "input1"); need_cuda_f32(input2, "input2"); need_cuda_f32(gradOutput, "gradOutput");
-    need_out(gradInput1, "gradInput1"); need_out(gradInput2, "gradInput2");
-    int rc;
-    {
-        c10::cuda::CUDAGuard guard(input1.device());
-        at::Tensor a = input1.contiguous(), b = input2.contiguous(), g = gradOutput.contiguous();
-        const int B = a.size(0), C = a.size(1), H = a.size(2), W = a.size(3);
-        gradInput1.resize_(a.sizes());       // :109-110
-        gradInput2.resize_(b.sizes());
-        const size_t ws = fn2b200_correlation_backward_workspace(B, C, H, W, pad_size, kernel_size, max_displacement, stride1, stride2);
-        at::Tensor wsb = scratch(ws, a);
-        rc = fn2b200_correlation_backward_ws(a.data_ptr<float>(), b.data_ptr<float>(), g.data_ptr<float>(),
-                                             gradInput1.data_ptr<float>(), gradInput2.data_ptr<float>(), B, C, H, W, pad_size,
-                                             kernel_size, max_displacement, stride1, stride2, corr_type_multiply,
-                                             ws ? wsb.data_ptr() : nullptr, ws, 0, stream_of(a));
-    }
-    check(rc, "correlation_backward");
+    need_cuda_f32(input1, "input1"); need_cuda_f32(input2, "input2"); need_cuda_f32(gradOutput, "grad_output");
+    need_cuda_f32(gradInput1, "grad_input1"); need_cuda_f32(gradInput2, "grad_input2");
+    gradInput1.resize_(input1.sizes());       // :109-110
+    gradInput2.resize_(input2.sizes());
+    // no workspace is handed over from the forward: the reference's Function keeps none
+    correlation_backward(input1, input2, gradOutput, false, std::nullopt, 0, 1.0, std::nullopt, pad_size, kernel_size,
+                         max_displacement, stride1, stride2, corr_type_multiply, true, true, gradInput1, gradInput2);
     return 1;
 }
 

@@ -4,43 +4,17 @@
 using namespace fn2ext;
 
 int resample2d_cuda_forward(at::Tensor &input1, at::Tensor &input2, at::Tensor &output, int kernel_size, bool bilinear) {
-    need_cuda_f32(input1, "input1"); need_cuda_f32(input2, "input2"); need_out(output, "output");
-    TORCH_CHECK(input1.dim() == 4 && input2.dim() == 4 && output.dim() == 4 && output.size(0) == input2.size(0) &&
-                output.size(1) == input1.size(1) && output.size(2) == input2.size(2) && output.size(3) == input2.size(3),
-                "output must be [B, C, H, W]");
-    int rc;
-    {
-        c10::cuda::CUDAGuard guard(input2.device());
-        at::Tensor flow = input2.contiguous();
-        const int64_t is[4] = {input1.stride(0), input1.stride(1), input1.stride(2), input1.stride(3)};
-        const int B = flow.size(0), C = input1.size(1), H = flow.size(2), W = flow.size(3);
-        rc = fn2b200_resample2d_forward(input1.data_ptr<float>(), is, flow.data_ptr<float>(), output.data_ptr<float>(), B, C,
-                                        (int)input1.size(2), (int)input1.size(3), H, W, kernel_size, bilinear ? 1 : 0,
-                                        stream_of(flow));
-    }
-    check(rc, "resample2d_forward");
+    need_cuda_f32(input1, "input1"); need_cuda_f32(input2, "input2"); need_cuda_f32(output, "output");
+    resample2d_forward(input1, input2, output, kernel_size, bilinear, 0, 1.0);
     return 1;
 }
 
 int resample2d_cuda_backward(at::Tensor &input1, at::Tensor &input2, at::Tensor &gradOutput, at::Tensor &gradInput1,
                              at::Tensor &gradInput2, int kernel_size, bool bilinear) {
-    need_cuda_f32(input1, "input1"); need_cuda_f32(input2, "input2"); need_cuda_f32(gradOutput, "gradOutput");
-    need_out(gradInput1, "gradInput1"); need_out(gradInput2, "gradInput2");
-    int rc;
-    {
-        c10::cuda::CUDAGuard guard(input2.device());
-        at::Tensor flow = input2.contiguous(), g = gradOutput.contiguous();
-        const int64_t is[4] = {input1.stride(0), input1.stride(1), input1.stride(2), input1.stride(3)};
-        const int B = flow.size(0), C = input1.size(1), H = flow.size(2), W = flow.size(3);
-        const int iH = input1.size(2), iW = input1.size(3);
-        const size_t ws = fn2b200_resample2d_backward_workspace(is, B, C, iH, iW, H, W);
-        at::Tensor wsb = scratch(ws, flow);
-        // zero_grad_input1 = 0: gradInput1 arrives zero-filled (resample2d.py:31) and is accumulated into
-        rc = fn2b200_resample2d_backward_ws(input1.data_ptr<float>(), is, flow.data_ptr<float>(), g.data_ptr<float>(),
-                                            gradInput1.data_ptr<float>(), gradInput2.data_ptr<float>(), B, C, iH, iW, H, W,
-                                            kernel_size, bilinear ? 1 : 0, 0, ws ? wsb.data_ptr() : nullptr, ws, stream_of(flow));
-    }
-    check(rc, "resample2d_backward");
+    need_cuda_f32(input1, "input1"); need_cuda_f32(input2, "input2"); need_cuda_f32(gradOutput, "grad_output");
+    need_cuda_f32(gradInput1, "grad_input1"); need_cuda_f32(gradInput2, "grad_input2");
+    // zero_grad_input1 = false: gradInput1 arrives zero-filled (resample2d.py:31) and is accumulated into
+    resample2d_backward(input1, input2, gradOutput, kernel_size, bilinear, true, true, gradInput1, gradInput2, false);
     return 1;
 }
 

@@ -6,9 +6,12 @@ extension modules of the same names (oracle/_ref) -- the parent test computes wh
 
     python tests/pybind_child.py ops
     python tests/pybind_child.py model <FlowNet2C|FlowNet2> <x.npy> <ref_out.npy>
-Prints one line starting with "OK" on success; any failure is an exception (non-zero exit).
+    python tests/pybind_child.py refusals
+Prints one line starting with "OK" on success (refusals: one JSON line, what tests/test_gpu_host_routes.py's cases give
+through the compiled modules); any failure is an exception (non-zero exit).
 """
 import faulthandler
+import json
 import os
 import sys
 
@@ -127,8 +130,16 @@ def model(name, x_path, ref_path):
     print("OK model %s rel_err_vs_reference_kernels=%.3e" % (name, e))
 
 
+def refusals():
+    compat.install("B1p")
+    from test_gpu_host_routes import ext_refusals
+    print(json.dumps(ext_refusals(*(sys.modules[n] for n in ("correlation_cuda", "resample2d_cuda", "channelnorm_cuda")))))
+
+
 if __name__ == "__main__":
     if sys.argv[1] == "ops":
         ops()
+    elif sys.argv[1] == "refusals":
+        refusals()
     else:
         model(sys.argv[2], sys.argv[3], sys.argv[4])
