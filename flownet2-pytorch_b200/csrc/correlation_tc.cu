@@ -11,16 +11,19 @@
 // fp32 accuracy on bf16 tensor cores: every operand is split x = hi + lo (two bf16, 16 significand
 // bits); S = hi*hi + hi*lo + lo*hi (3 MMAs, fp32 accumulate in registers), dropped lo*lo ~ 2^-18 relative.
 //
-// Forward pipeline (one persistent CTA per SM, warp-specialised, 288 threads):
+// Forward pipeline (one persistent CTA per SM, warp-specialised, 384 threads):
 //   prepass kernel : NCHW fp32 -> [n][class][yc][xc][c] bf16 hi / lo (channels contiguous = K-major)
-//   warp 8         : TMA producer: f1 tile  -> smem A [hi|lo][C/64][128 rows x 128 B]  (resident for the tile's units)
+//   warps 8-11     : TMA producer (one lane of warp 8):
+//                                  f1 tile  -> smem A [hi|lo][C/64][128 rows x 128 B]  (resident for the tile's units)
 //                                  f2 units -> smem B ring, one slot = hi OR lo of a unit x 64 channels
 //                    [144 rows x 128 B] = one 18-KB box, 128-byte swizzle; halo outside the image = TMA
 //                    out-of-bounds zero fill = the layer's zero padding
-//   warps 0-7      : two warpgroups, one per 64 tile pixels: wgmma m64n144k16 (hi slot: hi*hi and lo*hi, lo slot:
-//                    hi*lo, 4 k-steps each) into an fp32 register accumulator; each warp then moves the band entries
-//                    of its fragment, scaled by 1/C, through a private shared-memory buffer to out[n][(tj,ti)][y][x],
-//                    16 pixels x 2 displacement planes per store instruction
+//   warps 0-7      : two warpgroups, ping-pong by unit: the k-th unit of a CTA is computed by warpgroup k & 1 for all
+//                    128 tile pixels, wgmma m64n144k16 per 64-pixel half (hi slot: hi*hi and lo*hi, lo slot: hi*lo,
+//                    4 k-steps each) into two fp32 register accumulators; each warp then moves the band entries of
+//                    its two fragment rows, scaled by 1/C, through a private shared-memory buffer to
+//                    out[n][(tj,ti)][y][x], 16 pixels x 2 displacement planes per store instruction, while the other
+//                    warpgroup's wgmmas for the next unit run
 #include "wgmma.cuh"
 #include <cuda_bf16.h>
 #include <stdlib.h>
@@ -39,7 +42,7 @@ constexpr int TC_MAXBST = 12;                  // B ring slots (one per hi / lo 
 constexpr int TC_DS = 2 * TC_DR + 1;           // 21
 constexpr int TC_ABLK = 128 * 128;             // bytes of one A k-block (128 rows x 128 B)
 constexpr int TC_BBLK = TC_N * 128;            // bytes of one B k-block (144 rows x 128 B)
-constexpr int TC_NBAR = 2 * TC_MAXKB + 2 * TC_MAXBST;
+constexpr int TC_NBAR = 2 * TC_MAXKB + 2 * TC_MAXBST + 2;    // A full / empty, B full / empty, the 2 turn barriers
 constexpr int TC_SMEM_MAX = 232448;            // 227 KB opt-in limit per CTA (sm_90)
 // Forward epilogue staging: each consumer warp transposes its band through a private buffer [ti][px] of its 16 tile
 // pixels, one displacement row ti every TC_SPITCH floats.  The pitch makes the fill conflict-free: for one
@@ -147,10 +150,27 @@ __device__ __forceinline__ bool tc_next_seg(int &tn, int &w, int full, int w1, T
     return false;
 }
 
-// Warps 0-7: two consumer warpgroups; warpgroup wg owns tile pixels [64 wg, 64 wg + 64) (tile rows 4 wg .. 4 wg + 3) and
-// keeps their m64 x n144 accumulator of the current unit in registers.  Warp 8: the TMA producer (one lane issues).
+// Ring slots [b, b + n) that the calling warpgroup does not read (B slots; in the forward also the A blocks of a
+// segment, as a ring of nkb slots): wait for each fill, then release it.  Releasing a slot before its fill has landed
+// would complete the previous phase, and a slot refilled before this warpgroup saw its current phase would make the
+// parity of its next wait on the slot ambiguous.
+__device__ __forceinline__ void tc_skip_slots(uint64_t *full, uint64_t *empty, uint32_t b, int n, int bst) {
+    for (int i = 0; i < n; ++i, ++b) {
+        const int s = b % bst;
+        mbar_wait(&full[s], (b / bst) & 1);
+        mbar_arrive(&empty[s]);
+    }
+}
+
+// Warps 0-7: two consumer warpgroups that take the CTA's units in turn (ping-pong): the k-th unit the CTA runs belongs
+// to warpgroup k & 1, which keeps the unit's two m64 x n144 accumulators (tile rows 0-3 and 4-7) in registers and then
+// stores the unit's band while the other warpgroup's wgmmas for unit k + 1 run.  Warps 8-11: the producer warpgroup, of
+// which one lane of warp 8 issues the TMA loads.  Register budgets (setmaxnreg) fill the 64 K register file: the two
+// accumulators alone are 144 registers, more than ptxas grants a thread of a 288-thread kernel without spilling.
 constexpr int TC_CONSUMERS = 256;
-constexpr int TC_THREADS = TC_CONSUMERS + 32;
+constexpr int TC_THREADS = TC_CONSUMERS + 128;
+constexpr int TC_REG_MMA = 232, TC_REG_PROD = 40;
+static_assert(128 * (2 * TC_REG_MMA + TC_REG_PROD) <= 65536, "register budgets exceed the register file");
 __global__ void __launch_bounds__(TC_THREADS, 1)
 corr_fwd_tc_kernel(const __grid_constant__ CUtensorMap m1h, const __grid_constant__ CUtensorMap m1l,
                    const __grid_constant__ CUtensorMap m2h, const __grid_constant__ CUtensorMap m2l,
@@ -175,20 +195,24 @@ corr_fwd_tc_kernel(const __grid_constant__ CUtensorMap m1h, const __grid_constan
     uint64_t *bars = reinterpret_cast<uint64_t *>(sB + bst * TC_BBLK);
     uint64_t *a_full = bars, *a_empty = bars + TC_MAXKB;
     uint64_t *b_full = bars + 2 * TC_MAXKB, *b_empty = b_full + TC_MAXBST;
+    uint64_t *turn = b_empty + TC_MAXBST;                     // [warpgroup]: the previous unit's wgmmas are issued
     float *stage = reinterpret_cast<float *>(bars + TC_NBAR);  // [consumer warp][TC_SBUF]
 
     if (tid == 0) {
         prefetch_tensormap(&m1h); prefetch_tensormap(&m1l);
         prefetch_tensormap(&m2h); prefetch_tensormap(&m2l);
+        // A: both warpgroups arrive once per segment; B: a slot has one reader, the warpgroup of its unit
         for (int i = 0; i < TC_MAXKB; ++i) { mbar_init(&a_full[i], 1); mbar_init(&a_empty[i], TC_CONSUMERS); }
-        for (int i = 0; i < TC_MAXBST; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], TC_CONSUMERS); }
+        for (int i = 0; i < TC_MAXBST; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], TC_CONSUMERS / 2); }
+        for (int i = 0; i < 2; ++i) mbar_init(&turn[i], TC_CONSUMERS / 2);
         fence_barrier_init();
     }
     __syncthreads();
 
-    if (warp == TC_CONSUMERS / 32) {
+    if (warp >= TC_CONSUMERS / 32) {
         // ===================== TMA producer =====================
-        if (lane == 0) {
+        setmaxnreg_dec<TC_REG_PROD>();
+        if (warp == TC_CONSUMERS / 32 && lane == 0) {
             uint32_t bcount = 0;
             int it = 0;
             const uint64_t pol = l2_policy_evict_last();
@@ -218,9 +242,10 @@ corr_fwd_tc_kernel(const __grid_constant__ CUtensorMap m1h, const __grid_constan
         }
     } else {
         // ===================== consumers: wgmma + epilogue =====================
+        setmaxnreg_inc<TC_REG_MMA>();
         const int wg = warp >> 2, wq = warp & 3;
-        // accumulator fragment: rows 16 wq + lane / 4 (+ 8) of the warpgroup = tile row 4 wg + wq, columns pxa (+ 8)
-        const int py_t = 4 * wg + wq, pxa = lane >> 2, q = lane & 3;
+        // accumulator fragment of half h: rows 16 wq + lane / 4 (+ 8) of the half = tile row 4 h + wq, columns pxa (+ 8)
+        const int pxa = lane >> 2, q = lane & 3;
         // store role: tile pixel sx of the fragment row, displacement column ti = t + sd of a store pair
         const int sx = lane & 15, sd = lane >> 4;
         float *sbuf = stage + warp * TC_SBUF;
@@ -229,82 +254,129 @@ corr_fwd_tc_kernel(const __grid_constant__ CUtensorMap m1h, const __grid_constan
         const float inv_nelems = 1.0f / (float)C;
         const long plane = (long)H * W;
         const bool act = leaky != 1.f;
-        uint32_t bcount = 0;
+        // Barrier phases.  Both warpgroups walk all segments and count every unit (k) and ring slot (bcount) of the CTA
+        // in the producer's order; each waits on and releases only the slots of its own units.  A wait for fill P of a
+        // slot is unambiguous only if fill P - 1 has landed (otherwise the slot's last completed phase, P - 2, has the
+        // parity waited for), and fill P - 1 may belong to the other warpgroup's unit.  So unit k starts only after the
+        // warpgroup of unit k - 1 has passed all of that unit's b_full waits: it then arrives on turn[k & 1], and by
+        // induction every fill of the units before k has landed.  turn[w] completes its j-th phase when unit 2 j + 1 - w
+        // has been issued, so unit k waits for phase ((k + 1) >> 1) - 1 of turn[k & 1]; unit 0 waits for phase -1, which
+        // a fresh barrier reports complete.  The turns alternate, so neither turn barrier can run a phase ahead of its
+        // waiter.  A fill P + 1 needs the reader's release of fill P, so a slot cannot run ahead of its reader either.
+        // A is resident for a segment and read by both warpgroups: each waits for a_full and arrives on a_empty once per
+        // segment and k-block, after its last unit of the segment, or at once if it has no unit there (a one-unit
+        // segment of the last round), so that its wait in the next segment again sees the phase before.
+        uint32_t bcount = 0, k = 0;
         int it = 0;
         TcSeg sg;
         for (int tn = blockIdx.x, w = w0; tc_next_seg(tn, w, full, w1, sg); ++it) {
             const int ua = sg.ua, ub = sg.ub;
             const TcTile T = tc_decode(sg.t, nxt, nyt);
-            const int yc = T.yc0 + py_t, xc = T.xc0 + sx;
-            const bool ok = (yc < Hc) && (xc < Wc);
-            float *ob = out + (long)T.n * out_bstride + (long)(2 * yc + T.py) * W + (2 * xc + T.px);
-            for (int u = ua; u < ub; ++u) {
-                float acc[TC_N / 2];
+            const int xc = T.xc0 + sx;
+            const int uf = ua + (int)((k ^ (uint32_t)wg) & 1u);       // this warpgroup's first unit of the segment
+            if (uf >= ub) tc_skip_slots(a_full, a_empty, (uint32_t)it * nkb, nkb, nkb);
+            for (int u = uf; u < ub; u += 2) {
+                const uint32_t ku = k + (uint32_t)(u - ua);
+                uint32_t b = bcount + (uint32_t)(u - ua) * 2 * nkb;
+                mbar_wait(&turn[wg], (((ku + 1) >> 1) & 1) ^ 1);
+                float acc[2][TC_N / 2];
 #pragma unroll
-                for (int i = 0; i < TC_N / 2; ++i) acc[i] = 0.f;
-                wgmma_fence_operands(acc);
-                int prev = -1, prev_a = -1;            // ring slot (and A block) read by the wgmma group in flight
-                for (int kb = 0; kb < nkb; ++kb) {
-                    if (u == ua) mbar_wait(&a_full[kb], it & 1);
-                    const uint64_t dh = wgmma_desc_k_sw128(smem_u32(sA + kb * TC_ABLK + wg * (TC_ABLK / 2)));
-                    const uint64_t dl = wgmma_desc_k_sw128(smem_u32(sAlo + kb * TC_ABLK + wg * (TC_ABLK / 2)));
+                for (int h = 0; h < 2; ++h) {
 #pragma unroll
-                    for (int hl = 0; hl < 2; ++hl, ++bcount) {
-                        const int s = bcount % bst;
-                        mbar_wait(&b_full[s], (bcount / bst) & 1);
-                        const uint64_t bd = wgmma_desc_k_sw128(smem_u32(sB + s * TC_BBLK));
-                        wgmma_fence();
-#pragma unroll
-                        for (int ks = 0; ks < TC_KB / 16; ++ks) {
-                            wgmma_m64n144k16_k(acc, dh + 2 * ks, bd + 2 * ks);             // hi x hi | hi x lo
-                            if (hl == 0) wgmma_m64n144k16_k(acc, dl + 2 * ks, bd + 2 * ks); // lo x hi
-                        }
-                        wgmma_commit();
-                        wgmma_wait<1>();
-                        if (prev >= 0) {
-                            mbar_arrive(&b_empty[prev]);
-                            if (prev_a >= 0) mbar_arrive(&a_empty[prev_a]);
-                        }
-                        prev = s;
-                        prev_a = (hl == 1 && u == ub - 1) ? kb : -1;       // A block free for the next segment
-                    }
+                    for (int i = 0; i < TC_N / 2; ++i) acc[h][i] = 0.f;
+                    wgmma_fence_operands(acc[h]);
                 }
-                wgmma_wait<0>();
-                wgmma_fence_operands(acc);
-                mbar_arrive(&b_empty[prev]);
-                if (prev_a >= 0) mbar_arrive(&a_empty[prev_a]);
+                // the unit's wgmmas into the halves h with live[h]; called with constants, so that no wgmma sits on a
+                // path of its own (ptxas would serialise them all)
+                auto mma = [&](const bool live0, const bool live1) {
+                    const bool live[2] = {live0, live1};
+                    int prev = -1, prev_a = -1;            // ring slot (and A block) read by the wgmma group in flight
+                    for (int kb = 0; kb < nkb; ++kb) {
+                        if (u == uf) mbar_wait(&a_full[kb], it & 1);
+                        // A descriptors of the two halves (tile rows 0-3, 4-7): hi, then lo
+                        uint64_t da[2][2];
+#pragma unroll
+                        for (int h = 0; h < 2; ++h) {
+                            da[0][h] = wgmma_desc_k_sw128(smem_u32(sA + kb * TC_ABLK + h * (TC_ABLK / 2)));
+                            da[1][h] = wgmma_desc_k_sw128(smem_u32(sAlo + kb * TC_ABLK + h * (TC_ABLK / 2)));
+                        }
+#pragma unroll
+                        for (int hl = 0; hl < 2; ++hl, ++b) {
+                            const int s = b % bst;
+                            mbar_wait(&b_full[s], (b / bst) & 1);
+                            const uint64_t bd = wgmma_desc_k_sw128(smem_u32(sB + s * TC_BBLK));
+                            wgmma_fence();
+                            // each accumulator: hi x hi | hi x lo, then (hi slot) lo x hi, k-step by k-step
+#pragma unroll
+                            for (int ks = 0; ks < TC_KB / 16; ++ks) {
+#pragma unroll
+                                for (int lo = 0; lo <= (hl == 0); ++lo)
+#pragma unroll
+                                    for (int h = 0; h < 2; ++h)
+                                        if (live[h]) wgmma_m64n144k16_k(acc[h], da[lo][h] + 2 * ks, bd + 2 * ks);
+                            }
+                            wgmma_commit();
+                            if (hl == 1 && kb == nkb - 1) mbar_arrive(&turn[wg ^ 1]);   // unit k + 1 may start
+                            wgmma_wait<1>();
+                            if (prev >= 0) {
+                                mbar_arrive(&b_empty[prev]);
+                                if (prev_a >= 0) mbar_arrive(&a_empty[prev_a]);
+                            }
+                            prev = s;
+                            prev_a = (hl == 1 && u + 2 >= ub) ? kb : -1;       // A block free for the next segment
+                        }
+                    }
+                    wgmma_wait<0>();
+                    wgmma_fence_operands(acc[0]);
+                    wgmma_fence_operands(acc[1]);
+                    mbar_arrive(&b_empty[prev]);
+                    if (prev_a >= 0) mbar_arrive(&a_empty[prev_a]);
+                };
+                // unit 0 only meets tile rows 0-3 and unit 6 only tile rows 4-7: the other half's products would only
+                // reach out-of-band columns, which are never stored
+                if (u == 0) mma(true, false);
+                else if (u == TC_NU - 1) mma(false, true);
+                else mma(true, true);
                 // accumulator column c = hrl * 36 + qx (halo row hrl of the unit, halo column qx) of tile pixel
                 // (py_t, px) is displacement (tj, ti) = (u * 4 + hrl - py_t, qx - px) - (10, 10), if inside the band.
-                // Per halo row, tj is the same for the whole warp (its fragment rows are one tile row), and each of
-                // its 16 pixels has exactly 21 in-band columns among the row's 36, so the warp's buffer [ti][px] is
-                // wholly rewritten by each pass.  Storing from the buffer writes 16 consecutive pixels of 2
+                // Per halo row, tj is the same for the whole warp (its fragment rows of a half are one tile row), and
+                // each of its 16 pixels has exactly 21 in-band columns among the row's 36, so the warp's buffer [ti][px]
+                // is wholly rewritten by each pass.  Storing from the buffer writes 16 consecutive pixels of 2
                 // displacement planes per instruction (2 lines), where storing from the fragment wrote one value
-                // per lane to up to 32 different planes.
-                const int tjb = u * TC_UR - py_t;
+                // per lane to up to 32 different planes.  A dead half has no displacement row in the band.
 #pragma unroll
-                for (int hrl = 0; hrl < TC_UR; ++hrl) {
-                    const int tj = tjb + hrl;
-                    if ((unsigned)tj >= (unsigned)TC_DS) continue;     // warp-uniform
+                for (int h = 0; h < 2; ++h) {
+                    const int py_t = 4 * h + wq, yc = T.yc0 + py_t;
+                    const bool ok = (yc < Hc) && (xc < Wc);
+                    float *ob = out + (long)T.n * out_bstride + (long)(2 * yc + T.py) * W + (2 * xc + T.px);
+                    const int tjb = u * TC_UR - py_t;
 #pragma unroll
-                    for (int i = TC_HW * hrl / 8; i <= (TC_HW * hrl + TC_HW - 1) / 8; ++i)
+                    for (int hrl = 0; hrl < TC_UR; ++hrl) {
+                        const int tj = tjb + hrl;
+                        if ((unsigned)tj >= (unsigned)TC_DS) continue;     // warp-uniform
 #pragma unroll
-                        for (int j = 0; j < 4; ++j) {
-                            const int x = pxa + 8 * (j >> 1);
-                            const int ti = 8 * i + 2 * q + (j & 1) - TC_HW * hrl - x;
-                            if ((unsigned)ti < (unsigned)TC_DS) {           // implies the column lies in halo row hrl
-                                float v = acc[4 * i + j] * inv_nelems;
-                                if (act) v = v > 0.f ? v : v * leaky;      // fused nn.LeakyReLU (FlowNetC.py:87), warp-uniform
-                                sbuf[ti * TC_SPITCH + x] = v;
+                        for (int i = TC_HW * hrl / 8; i <= (TC_HW * hrl + TC_HW - 1) / 8; ++i)
+#pragma unroll
+                            for (int j = 0; j < 4; ++j) {
+                                const int x = pxa + 8 * (j >> 1);
+                                const int ti = 8 * i + 2 * q + (j & 1) - TC_HW * hrl - x;
+                                if ((unsigned)ti < (unsigned)TC_DS) {           // implies the column lies in halo row hrl
+                                    float v = acc[h][4 * i + j] * inv_nelems;
+                                    if (act) v = v > 0.f ? v : v * leaky;      // fused nn.LeakyReLU (FlowNetC.py:87), warp-uniform
+                                    sbuf[ti * TC_SPITCH + x] = v;
+                                }
                             }
-                        }
-                    __syncwarp();
-                    float *o = ob + (long)(tj * TC_DS + sd) * plane;
+                        __syncwarp();
+                        float *o = ob + (long)(tj * TC_DS + sd) * plane;
 #pragma unroll
-                    for (int t = 0; t < TC_DS; t += 2)
-                        if (ok && t + sd < TC_DS) __stcs(o + (long)t * plane, sbuf[(t + sd) * TC_SPITCH + sx]);
-                    __syncwarp();                                   // read before the next pass overwrites
+                        for (int t = 0; t < TC_DS; t += 2)
+                            if (ok && t + sd < TC_DS) __stcs(o + (long)t * plane, sbuf[(t + sd) * TC_SPITCH + sx]);
+                        __syncwarp();                                   // read before the next pass overwrites
+                    }
                 }
             }
+            k += (uint32_t)(ub - ua);
+            bcount += (uint32_t)(ub - ua) * 2 * nkb;
         }
     }
 }
@@ -379,17 +451,6 @@ template <> __device__ __forceinline__ void wgmma_bwd<3>(float (&d)[96], uint64_
 template <> __device__ __forceinline__ void wgmma_bwd<4>(float (&d)[128], uint64_t da, uint64_t db) {
     wgmma_m64n128k16_mn(*reinterpret_cast<float (*)[64]>(&d[0]), da, db);
     wgmma_m64n128k16_mn(*reinterpret_cast<float (*)[64]>(&d[64]), da, db + ((2 * TB_GBLK) >> 4));
-}
-
-// Ring slots [b, b + n) that the calling warpgroup does not read: wait for each fill, then release it.  Releasing a
-// slot before its fill has landed would complete the previous phase, and a slot refilled before this warpgroup saw its
-// current phase would make the parity of its next wait on the slot ambiguous.
-__device__ __forceinline__ void tc_skip_slots(uint64_t *full, uint64_t *empty, uint32_t b, int n, int bst) {
-    for (int i = 0; i < n; ++i, ++b) {
-        const int s = b % bst;
-        mbar_wait(&full[s], (b / bst) & 1);
-        mbar_arrive(&empty[s]);
-    }
 }
 
 // Both gradients in ONE launch: global tiles [t_begin, t_end) of [0, 2 ntiles).  One gradient only: tile g < ntiles
