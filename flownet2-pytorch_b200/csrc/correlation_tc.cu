@@ -150,8 +150,8 @@ __device__ __forceinline__ bool tc_next_seg(int &tn, int &w, int full, int w1, T
     return false;
 }
 
-// Ring slots [b, b + n) that the calling warpgroup does not read (B slots; in the forward also the A blocks of a
-// segment, as a ring of nkb slots): wait for each fill, then release it.  Releasing a slot before its fill has landed
+// Ring slots [b, b + n) that the calling warpgroup does not read (the forward's A blocks of a segment without a unit of
+// the warpgroup, as a ring of nkb slots): wait for each fill, then release it.  Releasing a slot before its fill has landed
 // would complete the previous phase, and a slot refilled before this warpgroup saw its current phase would make the
 // parity of its next wait on the slot ambiguous.
 __device__ __forceinline__ void tc_skip_slots(uint64_t *full, uint64_t *empty, uint32_t b, int n, int bst) {
@@ -398,6 +398,9 @@ corr_fwd_tc_kernel(const __grid_constant__ CUtensorMap m1h, const __grid_constan
 // One builder thread per tile pixel: all 4 halo rows x 21 displacements of the unit.  Loads stay coalesced (lanes =
 // pixels, one displacement plane per instruction); the band positions a pixel writes are the same for every unit, so
 // the zero columns of A are written ONCE at kernel start.
+// Epilogue: each MMA warp stores its tile row's 16 pixels x C channels, scaled by 1/C, 16 pixels x 2 channel planes per
+// store instruction (a register swap between lane pairs, no shared memory).  Each warpgroup releases only the
+// ring slots it reads, so one warpgroup's stores run under the other's wgmmas (phases: at the MMA warpgroups' loop).
 // ------------------------------------------------------------------------------------------------
 constexpr int TB_AHL = TC_N * 128;                 // 18432 B: hi (or lo) of a warpgroup's A, [k][64 pixels] (MN-major, SW128)
 constexpr int TB_ASTG = 2 * TB_AHL;                // hi + lo
@@ -408,8 +411,8 @@ __host__ __device__ constexpr uint32_t tb_a_offset(uint32_t p, uint32_t k) {
     return k * 128u + ((((p >> 3) ^ (k & 7u))) << 4) + (p & 7u) * 2u;
 }
 constexpr int TB_MAXBST = 6;
-// B ring full / empty, then A full [warpgroup][buffer], A empty [warpgroup][buffer]
-constexpr int TB_NBAR = 2 * TB_MAXBST + 2 * 2 * TB_NAST;
+// B ring full / empty, A full [warpgroup][buffer], A empty [warpgroup][buffer], then the 2 turn barriers
+constexpr int TB_NBAR = 2 * TB_MAXBST + 2 * 2 * TB_NAST + 2;
 // B staging: the unit's 144 K indices in 3 groups of 48 (12 halo columns x 4 rows); one ring slot = the hi (or the lo)
 // copy of one group x ALL channel blocks = up to 4 boxes of 6 KB, so one k-step covers N = C columns.
 constexpr int TB_NG = 3, TB_GW = TC_HW / TB_NG, TB_GK = TC_UR * TB_GW;   // 3 groups, 12 columns, 48 K
@@ -474,6 +477,7 @@ corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constan
     uint64_t *bars = reinterpret_cast<uint64_t *>(sB + bst * TB_BSTAGE);
     uint64_t *b_full = bars, *b_empty = bars + TB_MAXBST;
     uint64_t *a_full = bars + 2 * TB_MAXBST, *a_empty = a_full + 2 * TB_NAST;
+    uint64_t *turn = a_empty + 2 * TB_NAST;             // [warpgroup]: the other warpgroup has passed its solo unit's waits
 
     const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
     const int Hc = H >> 1, Wc = W >> 1;
@@ -488,6 +492,7 @@ corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constan
         prefetch_tensormap(&m1h); prefetch_tensormap(&m1l);
         for (int i = 0; i < TB_MAXBST; ++i) { mbar_init(&b_full[i], 1); mbar_init(&b_empty[i], TC_CONSUMERS); }
         for (int i = 0; i < 2 * TB_NAST; ++i) { mbar_init(&a_full[i], 64); mbar_init(&a_empty[i], 128); }
+        for (int i = 0; i < 2; ++i) mbar_init(&turn[i], 128);
         fence_barrier_init();
     }
     // columns of A outside a pixel row's band are zero for every unit: written once, here
@@ -645,8 +650,23 @@ corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constan
     const uint32_t aw32 = smem_u32(sA + wg * TB_NAST * TB_ASTG);
     uint64_t *full = a_full + wg * TB_NAST, *empty = a_empty + wg * TB_NAST;
     const float inv_nelems = 1.0f / (float)C;
-    uint32_t bcount = 0, ucount = 0;
-    for (int g = t_begin + blockIdx.x; g < t_end; g += gridDim.x) {
+    // Barrier phases.  Units 1-5 of a tile are read by both warpgroups; unit 0 only by warpgroup 0 and unit 6 only by
+    // warpgroup 1.  That is each warpgroup's solo unit su, whose ring slots it releases alone, with 2 arrivals per thread.
+    // Both warpgroups count every ring slot (bcount) in the producer's order.  A wait for fill P of a slot is
+    // unambiguous only if fill P - 1 has landed (otherwise the slot's last completed phase, P - 2, has the parity
+    // waited for), and a warpgroup does not see the fills of the other one's solo unit.  So each waits, before its
+    // first unit of a tile, until the other has passed all its b_full waits of the solo unit just before: warpgroup 1
+    // before unit 1 of tile it for warpgroup 0's unit 0 of tile it, warpgroup 0 before unit 0 of tile it for
+    // warpgroup 1's unit 6 of tile it - 1.  turn[w] completes its j-th phase when the other warpgroup has passed the
+    // waits of its j-th solo unit, so warpgroup 1 waits for phase it of turn[1] and warpgroup 0 for phase it - 1 of
+    // turn[0]; the first tile's phase -1 is one a fresh barrier reports complete.  Neither turn barrier can run a phase
+    // ahead of its waiter: its next phase needs the other warpgroup to pass its own turn wait, which needs this
+    // warpgroup's arrival after the wait.  A fill P + 1 needs the readers' release of fill P, so a slot cannot run
+    // ahead of a reader either.  These waits are the only coupling, so warpgroup 0's gradient stores run under
+    // warpgroup 1's unit 6, and warpgroup 1's under warpgroup 0's unit 0 of the next tile and the start of its unit 1.
+    const int su = wg * (TC_NU - 1);
+    uint32_t bcount = 0, ucount = 0, it = 0;
+    for (int g = t_begin + blockIdx.x; g < t_end; g += gridDim.x, ++it) {
         const bool second = both ? (g & 1) : (g >= ntiles);           // gradInput2 tile (block-uniform)
         const TcTile T = tc_decode(both ? (g >> 1) : (second ? g - ntiles : g), nxt, nyt);
         float acc[C / 2];
@@ -654,18 +674,19 @@ corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constan
         for (int i = 0; i < C / 2; ++i) acc[i] = 0.f;
         wgmma_fence_operands(acc);
         int prev = -1, prev_a = -1;                            // ring slot (and A buffer) read by the wgmma group in flight
-        // Warpgroup 1 releases unit 0's slots once the A of unit 1 is built, warpgroup 0 unit 6's after its epilogue.
-        if (wg == 1) bcount += 2 * TB_NG;
+        uint32_t prev_n = 1;                                   // arrivals that release it: 2 in the solo unit
+        if (wg == 1) bcount += 2 * TB_NG;                      // unit 0: warpgroup 0's alone
         for (int u = wg; u < TC_NU - 1 + wg; ++u, ++ucount) {
             const int ab = ucount & 1;
             mbar_wait(&full[ab], (ucount >> 1) & 1);
-            if (u == 1 && wg == 1) tc_skip_slots(b_full, b_empty, bcount - 2 * TB_NG, 2 * TB_NG, bst);
+            if (u == wg) mbar_wait(&turn[wg], (it & 1) ^ (uint32_t)wg ^ 1u);
             const uint32_t ah32 = aw32 + ab * TB_ASTG, al32 = ah32 + TB_AHL;
             for (int gr = 0; gr < TB_NG; ++gr)
 #pragma unroll
                 for (int hl = 0; hl < 2; ++hl, ++bcount) {
                     const int s = bcount % bst;
                     mbar_wait(&b_full[s], (bcount / bst) & 1);
+                    if (u == su && gr == TB_NG - 1 && hl == 1) mbar_arrive(&turn[wg ^ 1]);   // the solo unit has landed
                     const uint32_t bb = smem_u32(sB + s * TB_BSTAGE);
                     wgmma_fence();
 #pragma unroll
@@ -678,30 +699,35 @@ corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constan
                     wgmma_commit();
                     wgmma_wait<1>();
                     if (prev >= 0) {
-                        mbar_arrive(&b_empty[prev]);
+                        mbar_arrive_cnt(&b_empty[prev], prev_n);
                         if (prev_a >= 0) mbar_arrive(&empty[prev_a]);
                     }
                     prev = s;
+                    prev_n = u == su ? 2u : 1u;
                     prev_a = (gr == TB_NG - 1 && hl == 1) ? ab : -1;   // the unit's last read of its A buffer
                 }
         }
         wgmma_wait<0>();
         wgmma_fence_operands(acc);
-        mbar_arrive(&b_empty[prev]);
+        mbar_arrive_cnt(&b_empty[prev], prev_n);
         mbar_arrive(&empty[prev_a]);
-        // epilogue: fragment rows = tile pixels (py_t, pxa) and (py_t, pxa + 8), columns = channels
-        const int yc = T.yc0 + py_t, xc = T.xc0 + pxa;
-        const bool ok0 = (yc < Hc) && (xc < Wc), ok1 = (yc < Hc) && (xc + 8 < Wc);
-        float *o = (second ? gin2 : gin1) + (long)T.n * C * plane + (long)(2 * yc + T.py) * W + (2 * xc + T.px);
+        if (wg == 0) bcount += 2 * TB_NG;                      // unit 6: warpgroup 1's alone
+        // epilogue: fragment rows = tile pixels (py_t, pxa) and (py_t, pxa + 8), columns = channels 8 i + 2 q (+ 1).  The
+        // lane pair q = 2 m, 2 m + 1 swaps halves (one shfl.xor per channel parity), so that lane q holds pixel
+        // sx = pxa + 8 (q & 1) of the four channels 8 i + 4 m + k; each store instruction then writes 16 consecutive
+        // tile pixels of 2 channel planes (2 lines), where storing the fragment as it is wrote 8 pixels of 4 planes.
+        const int sx = pxa + 8 * (q & 1), yc = T.yc0 + py_t, xc = T.xc0 + sx;
+        const bool ok = (yc < Hc) && (xc < Wc), odd = q & 1;
+        float *o = (second ? gin2 : gin1) + ((long)T.n * C + 4 * (q >> 1)) * plane + (long)(2 * yc + T.py) * W + (2 * xc + T.px);
 #pragma unroll
-        for (int i = 0; i < C / 8; ++i)
+        for (int i = 0; i < C / 8; ++i) {
+            const float *a = acc + 4 * i;          // [pixel half][channel parity] of channels 8 i + 2 q (+ 1)
+            const float r0 = __shfl_xor_sync(0xffffffffu, odd ? a[0] : a[2], 1);
+            const float r1 = __shfl_xor_sync(0xffffffffu, odd ? a[1] : a[3], 1);
+            const float v[4] = {odd ? r0 : a[0], odd ? r1 : a[1], odd ? a[2] : r0, odd ? a[3] : r1};
 #pragma unroll
-            for (int j = 0; j < 4; ++j)
-                if ((j >> 1) ? ok1 : ok0)
-                    __stcs(o + 16 * (j >> 1) + (long)(8 * i + 2 * q + (j & 1)) * plane, acc[4 * i + j] * inv_nelems);
-        if (wg == 0) {
-            tc_skip_slots(b_full, b_empty, bcount, 2 * TB_NG, bst);
-            bcount += 2 * TB_NG;
+            for (int k = 0; k < 4; ++k)
+                if (ok) __stcs(o + (long)(8 * i + k) * plane, v[k] * inv_nelems);
         }
     }
 }

@@ -90,6 +90,10 @@ __device__ __forceinline__ void wgmma_m64n192k16_mn(float (&d)[96], uint64_t da,
 __device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
     asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
+// n arrivals at once (a reader that stands in for a second one)
+__device__ __forceinline__ void mbar_arrive_cnt(uint64_t *bar, uint32_t n) {
+    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(n) : "memory");
+}
 // 2D tiled TMA load (any element type; swizzle comes from the tensor map)
 __device__ __forceinline__ void tma_load_2d(void *dst, const CUtensorMap *map, uint64_t *bar, int c0,
                                             int c1) {
