@@ -1,4 +1,5 @@
-"""Opt-in fused forwards for the reference's FlowNetC / FlowNet2C / FlowNet2 (SURVEY 8f rows 1-3).
+"""Opt-in fused forwards for the reference's FlowNetC / FlowNet2C / FlowNet2CS / FlowNet2CSS / FlowNet2 (SURVEY 8f
+rows 1-3).
 
 The drop-in modules (``Correlation``, ``Resample2d``, ``ChannelNorm``) keep the reference's module graph: each layer
 reads and writes whole tensors, and ``models.py`` glues them with ``nn.Upsample``, a subtraction, a division and
@@ -11,6 +12,8 @@ and hyper-parameters are used as they are) and run the same data flow with the g
 * ``flownet2_forward``  -- models.py:120-185: every ``upsample -> Resample2d -> diff -> ChannelNorm -> cat`` group is
   ONE kernel (``functional.warp_concat_forward``, 8f-1) that reads the quarter-resolution flow directly (8f-3) and writes
   the concat buffer the next sub-network consumes.
+* ``fused_forward`` on a FlowNet2CS / FlowNet2CSS -- models.py:392-416 / :469-505: the first one / two stages of the
+  same data flow (``_stacked_flow2``, shared with FlowNet2), then the network's own output ``nn.Upsample``.
 
 ``flownetc_forward``, ``flownet2c_forward``, ``flownet2_forward`` and ``fused_forward`` are inference only
 (``torch.no_grad`` is entered there).  For training:
@@ -21,8 +24,11 @@ and hyper-parameters are used as they are) and run the same data flow with the g
   LeakyReLU's derivative from the saved concat (conv3_1 keeps it alive anyway): no masked copy of the cost volume, no
   separate correlation output kept for backward.  Gradients are bit-identical to the unfused
   ``Correlation`` -> ``LeakyReLU`` -> ``torch.cat`` graph.
-* ``train_forward(net, inputs)`` -- FlowNetC / FlowNet2C with autograd on, through ``CorrelationCat``; returns what
-  ``net.forward`` returns in the net's current mode (flow2..flow6 in training).  FlowNet2 has its own entry point:
+* ``train_forward(net, inputs)`` -- FlowNetC / FlowNet2C / FlowNet2CS / FlowNet2CSS with autograd on, through
+  ``CorrelationCat`` (and for CS / CSS ``WarpConcat(upsample="bilinear")`` for concat1 / concat2); returns what
+  ``net.forward`` returns in the net's current mode (flow2..flow6 for FlowNetC / FlowNet2C in training, CS / CSS's
+  full-resolution flow in either mode).  ``fused_forward`` on a CS / CSS is this function under ``torch.no_grad``.
+  FlowNet2 has its own entry point:
 * ``flownet2_train_forward(net, inputs)`` -- FlowNet2 with autograd on: ``CorrelationCat`` in the FlowNetC stage,
   ``WarpConcat(upsample="bilinear")`` for concat1 / concat2 and ``FusionConcat`` for concat3.  ``flownet2_forward`` is
   this function under ``torch.no_grad``, so inference and training share one data flow.
@@ -192,26 +198,32 @@ def flownet2c_forward(net, inputs):
         return net.upsample1(flow2 * net.div_flow)
 
 
+def _stacked_flow2(net, inputs, n_s):
+    """The C -> S1 -> S2 branch FlowNet2, FlowNet2CS and FlowNet2CSS share (models.py:120-150, :392-413, :469-502),
+    differentiable when grad mode is on: FlowNetC through CorrelationCat, then the n_s FlowNetS stages
+    net.flownets_1 .. net.flownets_<n_s>, each fed by concat = (x | img1 warped | flow / div_flow | |img0 - warped|) of
+    the previous stage's flow through WarpConcat(upsample="bilinear").  Returns (x, the last stage's quarter-resolution
+    flow2)."""
+    div = float(net.div_flow)
+    x = _normalise(inputs, net.rgb_max)
+    x = torch.cat((x[:, :, 0], x[:, :, 1]), dim=1).float()
+    flow2 = _flownetc_pair(net.flownetc, x[:, 0:3], x[:, 3:])[0]
+    for i in range(1, n_s + 1):
+        concat = warp_concat(x, flow2, div, upsample="bilinear")
+        flow2 = getattr(net, "flownets_%d" % i)(concat)[0]
+        del concat
+    return x, flow2
+
+
 def flownet2_train_forward(net, inputs):
     """models.FlowNet2.forward (models.py:120-185) with the warp groups fused, differentiable when grad mode is on.
     net: the reference's FlowNet2; inputs [B,3,2,H,W].  Returns what net.forward returns (flownetfusion's flow).
     The FlowNetC stage runs through CorrelationCat, concat1 / concat2 through WarpConcat(upsample="bilinear") and
     concat3 through FusionConcat: neither the x4 upsampled flows nor their gradients are materialised."""
-    div = float(net.div_flow)
-    x = _normalise(inputs, net.rgb_max)
-    x = torch.cat((x[:, :, 0], x[:, :, 1]), dim=1).float()
-    # flownetc -> concat1 = (x | img1 warped | flow / div_flow | |img0 - warped|)                models.py:129-138
-    flow2 = _flownetc_pair(net.flownetc, x[:, 0:3], x[:, 3:])[0]
-    concat1 = warp_concat(x, flow2, div, upsample="bilinear")
-    # flownets1 -> concat2                                                                        models.py:141-150
-    flow2 = net.flownets_1(concat1)[0]
-    concat2 = warp_concat(x, flow2, div, upsample="bilinear")
-    del concat1
-    # flownets2 and flownetsd -> concat3 = (img0 | sd flow | s2 flow | their norms | the two diff norms)       :153-179
-    s2_flow2 = net.flownets_2(concat2)[0]
-    del concat2
+    x, s2_flow2 = _stacked_flow2(net, inputs, 2)
+    # flownetsd -> concat3 = (img0 | sd flow | s2 flow | their norms | the two diff norms)         models.py:153-179
     sd_flow2 = net.flownets_d(x)[0]
-    return net.flownetfusion(fusion_concat(x, sd_flow2, s2_flow2, div))
+    return net.flownetfusion(fusion_concat(x, sd_flow2, s2_flow2, float(net.div_flow)))
 
 
 def flownet2_forward(net, inputs):
@@ -222,26 +234,38 @@ def flownet2_forward(net, inputs):
 
 
 def fused_forward(net, inputs):
-    """Dispatch on the reference class name: FlowNet2, FlowNet2C or a bare FlowNetC."""
+    """Dispatch on the reference class name: FlowNet2, FlowNet2CSS, FlowNet2CS, FlowNet2C or a bare FlowNetC
+    (inference, torch.no_grad)."""
     name = type(net).__name__
     if name == "FlowNet2":
         return flownet2_forward(net, inputs)
+    if name in ("FlowNet2CS", "FlowNet2CSS"):
+        with torch.no_grad():
+            return train_forward(net, inputs)
     if name == "FlowNet2C":
         return flownet2c_forward(net, inputs)
     if name == "FlowNetC":
         return flownetc_forward(net, inputs)
-    raise TypeError("fused_forward: no fused data flow for %s (FlowNet2, FlowNet2C, FlowNetC)" % name)
+    raise TypeError("fused_forward: no fused data flow for %s (FlowNet2, FlowNet2CSS, FlowNet2CS, FlowNet2C, FlowNetC)"
+                    % name)
 
 
 def train_forward(net, inputs):
     """net.forward with autograd, with the correlation -> LeakyReLU -> concat of FlowNetC fused (CorrelationCat).
-    net: the reference's FlowNetC (inputs [B,6,H,W]) or FlowNet2C (inputs [B,3,2,H,W]).  Returns what net.forward
-    returns in the net's current mode: (flow2, flow3, flow4, flow5, flow6) when net.training (FlowNetC.py:125-128,
-    models.py:250-253), else FlowNetC's (flow2,) / FlowNet2C's upsample1(flow2 * div_flow)."""
+    net: the reference's FlowNetC (inputs [B,6,H,W]), FlowNet2C, FlowNet2CS or FlowNet2CSS (inputs [B,3,2,H,W]).
+    Returns what net.forward returns in the net's current mode: (flow2, flow3, flow4, flow5, flow6) when net.training
+    (FlowNetC.py:125-128, models.py:250-253), else FlowNetC's (flow2,) / FlowNet2C's upsample1(flow2 * div_flow).
+    FlowNet2CS / FlowNet2CSS return their full-resolution flow in either mode (models.py:414-416, :503-505): the last
+    FlowNetS stage's flow2 from _stacked_flow2, times div_flow, through the network's own upsample2 / upsample3."""
     name = type(net).__name__
     if name == "FlowNet2":
         raise TypeError("train_forward: FlowNet2 has no differentiable fused data flow here (train_forward covers "
-                        "FlowNetC and FlowNet2C); use fused.flownet2_train_forward(net, inputs)")
+                        "FlowNetC, FlowNet2C, FlowNet2CS and FlowNet2CSS); use "
+                        "fused.flownet2_train_forward(net, inputs)")
+    if name == "FlowNet2CS":
+        return net.upsample2(_stacked_flow2(net, inputs, 1)[1] * net.div_flow)
+    if name == "FlowNet2CSS":
+        return net.upsample3(_stacked_flow2(net, inputs, 2)[1] * net.div_flow)
     if name == "FlowNet2C":
         x = _normalise(inputs, net.rgb_max)
         flows = _flownetc_pair(net, x[:, :, 0], x[:, :, 1])
@@ -249,4 +273,4 @@ def train_forward(net, inputs):
     if name == "FlowNetC":
         flows = _flownetc_pair(net, inputs[:, 0:3], inputs[:, 3:])
         return flows if net.training else flows[:1]
-    raise TypeError("train_forward: no fused data flow for %s (FlowNet2C, FlowNetC)" % name)
+    raise TypeError("train_forward: no fused data flow for %s (FlowNet2CSS, FlowNet2CS, FlowNet2C, FlowNetC)" % name)
