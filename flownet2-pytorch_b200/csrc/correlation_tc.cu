@@ -9,7 +9,8 @@
 //        S[p, q] = sum_c f1[c, p] * f2[c, q]        (p in tile, q in halo),
 // computed as a GEMM in 7 "units" of 4 halo rows (N = 144 columns) over K = C channels.
 // fp32 accuracy on bf16 tensor cores: every operand is split x = hi + lo (two bf16, 16 significand
-// bits); S = hi*hi + hi*lo + lo*hi (3 MMAs, fp32 accumulate in registers), dropped lo*lo ~ 2^-18 relative.
+// bits); S = hi*hi + hi*lo + lo*hi (3 MMAs, fp32 accumulate in registers), dropped lo*lo ~ 2^-18 relative
+// (tc_split_hi: finite x splits into finite halves, the bf16 overflow window included).
 //
 // Forward pipeline (one persistent CTA per SM, warp-specialised, 384 threads):
 //   prepass kernel : NCHW fp32 -> [n][class][yc][xc][c] bf16 hi / lo (channels contiguous = K-major)
@@ -56,6 +57,17 @@ __host__ __device__ constexpr int tc_smem_bytes(int nkb, int bst) {
     return 2 * nkb * TC_ABLK + bst * TC_BBLK + TC_NBAR * 8 + 8 * TC_SBUF * 4 + 1024;
 }
 
+// The hi half of the split x = hi + lo: rn_bf16(x), saturated to the largest finite bf16.  A finite x in the bf16
+// overflow window (|x| in [0x7F7F8000, 0x7F7FFFFF]) would round to a bf16 infinity and make lo = -inf; saturated, lo =
+// rn(x - hi) stays finite and |x - hi - lo| <= 2^-16 |x| still holds.  ±inf splits into (±max, ±inf) and NaN into NaN.
+// One cvt.satfinite replaces the cvt.rn: a window test beside it added six instructions per gradOutput value to the
+// backward's builder and slowed corr_bwd_tc_kernel by ~6 %.
+__device__ __forceinline__ __nv_bfloat16 tc_split_hi(float x) {
+    unsigned short h;
+    asm("cvt.rn.satfinite.bf16.f32 %0, %1;" : "=h"(h) : "f"(x));
+    return __ushort_as_bfloat16(h);
+}
+
 // ------------------------------------------------------------------------------------------------
 // Prepass: NCHW fp32 -> parity-class-separated NHWC bf16 hi / lo
 // ------------------------------------------------------------------------------------------------
@@ -97,7 +109,7 @@ corr_tc_split_kernel(const float *__restrict__ in0, const float *__restrict__ in
         for (int i = 0; i < 8; ++i) {
             const int c = (i >> 2) * 32 + cg * 8 + 2 * (i & 3);
             const float v0 = tile[c][xo], v1 = tile[c + 1][xo];
-            const __nv_bfloat16 h0 = __float2bfloat16_rn(v0), h1 = __float2bfloat16_rn(v1);
+            const __nv_bfloat16 h0 = tc_split_hi(v0), h1 = tc_split_hi(v1);
             const __nv_bfloat16 l0 = __float2bfloat16_rn(v0 - __bfloat162float(h0));
             const __nv_bfloat16 l1 = __float2bfloat16_rn(v1 - __bfloat162float(h1));
             hw[i] = (uint32_t)__bfloat16_as_ushort(h0) | ((uint32_t)__bfloat16_as_ushort(h1) << 16);
@@ -629,7 +641,7 @@ corr_bwd_tc_kernel(const __grid_constant__ CUtensorMap m2h, const __grid_constan
                 for (int h = 0; h < TC_UR; ++h)
 #pragma unroll
                     for (int j = 0; j < TC_DS; ++j) {
-                        const __nv_bfloat16 hv = __float2bfloat16_rn(v[h][j]);
+                        const __nv_bfloat16 hv = tc_split_hi(v[h][j]);
                         const __nv_bfloat16 lv = __float2bfloat16_rn(v[h][j] - __bfloat162float(hv));
                         const uint32_t o = tb_row_offset((ao[j / 2] >> (16 * (j & 1))) & 0xFFFFu, h);
                         *reinterpret_cast<unsigned short *>(ah + o) = __bfloat16_as_ushort(hv);

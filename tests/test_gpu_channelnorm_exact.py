@@ -22,10 +22,10 @@ import ctypes
 
 import pytest
 import torch
-from torch.profiler import ProfilerActivity, profile
 
 import torch_ref
 from guarded import Arena
+from util import cuda_profile
 
 pytestmark = pytest.mark.gpu
 P = ctypes.c_void_p
@@ -106,7 +106,7 @@ def _run(x, go, misalign, want):
     # the profiler can drop the record of a kernel that ran: a missing name runs the (deterministic) calls once more
     ran = set()
     for _ in range(2):
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        with cuda_profile() as prof:
             launch()
             torch.cuda.synchronize()
         ran |= _kernels(prof)

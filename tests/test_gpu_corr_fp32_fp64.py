@@ -64,10 +64,10 @@ import ctypes
 
 import pytest
 import torch
-from torch.profiler import ProfilerActivity, profile
 
 import torch_ref
 from guarded import SENTINEL, Arena
+from util import cuda_profile
 
 pytestmark = pytest.mark.gpu
 P = ctypes.c_void_p
@@ -211,7 +211,7 @@ def _profiled(call, want):
     profiler and the kernels of both records count."""
     names = set()
     for attempt in range(2):
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        with cuda_profile() as prof:
             res = call()
             torch.cuda.synchronize()
         names |= {e.name for e in prof.events() if e.device_type == torch.autograd.DeviceType.CUDA and "corr" in e.name}

@@ -17,14 +17,13 @@ import ctypes
 import numpy as np
 import pytest
 import torch
-from torch.profiler import ProfilerActivity, profile
 
 import torch_ref
 import upsample_ref as ur
 from guarded import SENTINEL, Arena
 from kernel_manifest import KERNELS
 from oracle import cpu as orc
-from util import assert_close
+from util import assert_close, cuda_profile
 
 pytestmark = pytest.mark.gpu
 P = ctypes.c_void_p
@@ -51,23 +50,26 @@ def _kernel_names(prof):
 
 @pytest.fixture(autouse=True)
 def launched_kernels(request, monkeypatch):
-    """Profiles the case; afterwards every instantiation the manifest assigns to it must have run.  A case that already
-    failed is not reported twice.  The profiler has been seen to lose the record of a kernel's first launch in the
-    process (twice in about a thousand cases, each time the launch that loaded the kernel), so a case whose record is
-    missing runs once more, its kernels now loaded, before it fails.  (Requesting monkeypatch keeps the environment the
-    case set until that second run is over.)"""
+    """Profiles the case (util.cuda_profile); afterwards every instantiation the manifest assigns to it must have run.
+    A case that already failed is not reported twice.  The profiler has been seen to lose the record of the first
+    kernel the library launches in a profiling session (a case's forward missing while its backward was recorded), so
+    a case whose record is missing runs twice more in one fresh session before it fails: every kernel of the second
+    run follows one already recorded.  (Requesting monkeypatch keeps the environment the case set until those runs are
+    over.)"""
     want = {k for k, v in KERNELS.items() if v == request.node.name}
     failed_before = request.session.testsfailed
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+    with cuda_profile() as prof:
         yield
         torch.cuda.synchronize()
     if request.session.testsfailed != failed_before or not (want - _kernel_names(prof)):
         return
-    with profile(activities=[ProfilerActivity.CUDA]) as prof:
-        request.node.runtest()
-        torch.cuda.synchronize()
+    with cuda_profile() as prof:
+        for _ in range(2):
+            request.node.runtest()
+            torch.cuda.synchronize()
     missing = want - _kernel_names(prof)
-    assert not missing, "%s did not launch %s" % (request.node.name, sorted(missing))
+    assert not missing, "%s did not launch %s; recorded %s" % (request.node.name, sorted(missing),
+                                                              sorted(_kernel_names(prof)))
 
 
 @pytest.fixture
